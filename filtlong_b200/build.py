@@ -1,6 +1,6 @@
-"""Builds libfiltlong_b200.so (hand-written sm_100a CUDA behind a C ABI) in-tree with nvcc.
+"""Builds libfiltlong_b200.so (hand-written sm_90a CUDA behind a C ABI) in-tree with nvcc.
 
-The shared object is git-ignored but travels to the GPU box with gpurun. No CPU fallback exists:
+The shared object is a build product, kept out of git. No CPU fallback exists:
 if the library is missing or cannot be loaded, importing filtlong_b200.capi raises.
 """
 import os
@@ -19,7 +19,7 @@ SYNTH_LIB = os.path.join(PKG, "libflsynth_host.so")
 CXX = os.environ.get("CXX", "g++")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # --fmad=false: the per-read scores must follow the reference's unfused double arithmetic
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "--fmad=false", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "--fmad=false", "-std=c++17",
          "-Xcompiler", "-fPIC,-O2,-ffp-contract=off", "-Xptxas", "-v"]
 
 
@@ -51,7 +51,7 @@ def build_library(force=False, verbose=False):
         if p.returncode != 0:
             raise RuntimeError("nvcc failed on %s" % src)
     if force or procs or _stale(LIB, objs):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-ldl"]
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + ["-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout + r.stderr)

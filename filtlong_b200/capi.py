@@ -1,6 +1,6 @@
 """ctypes binding of libfiltlong_b200.so (include/filtlong_b200.h).
 
-This is the only way Python reaches the hot path: every call lands in the hand-written sm_100a
+This is the only way Python reaches the hot path: every call lands in the hand-written sm_90a
 CUDA library through its C ABI. There is no CPU or PyTorch fallback -- if the shared object is
 missing, or no CUDA device is usable, the error is raised to the caller.
 """

@@ -11,7 +11,7 @@ static void drain_timers(fl_ctx *c);
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
-extern "C" const char *fl_version(void) { return "filtlong-b200 0.1 (Filtlong v0.3.1 semantics, sm_100a)"; }
+extern "C" const char *fl_version(void) { return "filtlong-b200 0.1 (Filtlong v0.3.1 semantics, sm_90a)"; }
 
 extern "C" const char *fl_last_error(const fl_ctx *ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -61,7 +61,7 @@ extern "C" int fl_ctx_create(const fl_params *params, int device, fl_ctx **out) 
         return FL_ECUDA;
     }
     c->stream = c->own_stream;
-    // tuning knobs for profiling runs (defaults are the measured best, see profiles/ and DESIGN.md section 7)
+    // tuning knobs for profiling runs (DESIGN.md section 4.2)
     if (const char *f = getenv("FL_FILTER")) c->filter_enabled = atoi(f);
     if (const char *f = getenv("FL_ANCHOR")) c->anchor_enabled = atoi(f);
     if (const char *f = getenv("FL_PHRED_MODE")) c->phred_mode = atoi(f);

@@ -1,4 +1,4 @@
-// filtlong_b200/csrc/fl_internal.cuh -- shared declarations of the CUDA library (sm_100a only).
+// filtlong_b200/csrc/fl_internal.cuh -- shared declarations of the CUDA library (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -127,7 +127,7 @@ struct fl_ctx {
     uint64_t n_kmers = 0;
     // optional L2-resident pre-filter of the set (built when the set is small enough to make it selective)
     unsigned long long *d_filter = nullptr;
-    unsigned filter_log2_words = 22;     // 2^22 x 8 B = 32 MiB (measured best on B200: 64 MiB no longer stays in L2)
+    unsigned filter_log2_words = 22;     // 2^22 x 8 B = 32 MiB (sizes: see filter_min_bits_per_key)
     // Flavour of the pre-filter (fl_device.cuh): bit 2 = one word per table group of four 16-mers; bit 3 = one word per pair
     // of neighbours; bit 4 = four bits per member instead of two (bits 0 and 1 are unused: former experiments). -1 = chosen
     // from the set's size when the set is finalised (fl_kmers_recount).
@@ -139,7 +139,11 @@ struct fl_ctx {
     bool use_anchor = false;
     int anchor_enabled = 1;              // FL_ANCHOR=0 probes the bitmap itself (profiling, cross-checks)
     int filter_enabled = 1;              // FL_FILTER=0 disables (profiling)
-    int filter_min_bits_per_key = 8;     // the filter is used while it has at least this many bits per member
+    // The filter is used while it has at least this many bits per member: 40 keeps it to sets of <= 6.7 M members (the
+    // group-keyed regime). Measured on an H100 80GB HBM3 at 400 W, config 3's set (20 M members) against 10 Gbp of reads,
+    // probe ms: no filter 84.8; pair-keyed 16 / 32 / 64 MiB 101.5 / 115.9 / 148.7; per 16-mer 32 / 64 MiB 194.7 / 279.4.
+    // Smaller sets were not measured on the H100.
+    int filter_min_bits_per_key = 40;
     bool kmers_count_stale = false;
     // multiple-copy build state (kmers.cpp:142-166 in closed form, see fl_kmers.cu)
     uint32_t *d_seen[4] = {nullptr, nullptr, nullptr, nullptr};   // ">= 1,2,3,4 sightings" bitmaps

@@ -1,7 +1,7 @@
 // filtlong_b200/csrc/fl_kmers.cu -- device-built, device-resident reference 16-mer set.
 //
 // Replaces Kmers (reference src/kmers.cpp:28-239). The key space is exactly 2^32, so membership is
-// a direct-address bitmap (512 MiB of the 180 GB HBM3e): no collisions, no rehash, one 32-byte
+// a direct-address bitmap (512 MiB of the 80 GB HBM3): no collisions, no rehash, one 32-byte
 // sector per probe. Two build modes:
 //
 //   one copy        (kmers.cpp:137-139, assembly):  every forward / reverse 16-mer -> atomicOr.
@@ -345,16 +345,15 @@ int fl_kmers_recount(fl_ctx *ctx) {
     FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->n_kmers = ctx->h_scalars[0];
     ctx->kmers_count_stale = false;
-    // The pre-filter pays off while it stays selective: <= 1 member per 8 filter bits (false-positive
-    // rate of the two-bit test below ~5 %). Larger sets (e.g. a 3 Gbp assembly fills 75 % of the key
-    // space) are probed directly.
+    // The pre-filter is used while it has filter_min_bits_per_key bits per member (fl_internal.cuh: on the H100 a 20 M-member
+    // set probes faster without it). Larger sets (config 3's, or a 3 Gbp assembly that fills 75 % of the key space) are
+    // probed directly.
     const size_t filter_words = (size_t)1 << ctx->filter_log2_words;
     ctx->use_filter = ctx->filter_enabled && ctx->n_kmers > 0 && ctx->n_kmers * (uint64_t)ctx->filter_min_bits_per_key <= filter_words * 64;
     // Which flavour: the probe kernel is bound by L1TEX sector look-ups on a sparse set, one per filter word it loads, so a
     // word shared by the four 16-mers of a table group (or by two neighbours) cuts them 4x (2x) -- at 4x (2x) the insertions.
-    // Small sets can afford that (false positives, each a wasted random HBM sector, stay below ~5 %). Measured, probe ms of
-    // config 3's reads against sets of 5 / 10 / 15 / 20 M members (profiles/r02_probe_variants4_filter_flavour_by_set_size.jsonl):
-    // per-16-mer 92 / 93 / - / 95, pair-keyed 66 / 68 / 76 / 87, group-keyed 64 / 77 / 100 / 109.
+    // Small sets can afford that (false positives, each a wasted random HBM sector, stay below ~5 %); the thresholds
+    // (filter_group4_max, filter_pair_max) come from a sweep of config 3's reads against sets of 5 to 20 M members.
     if (ctx->filter_kind_request >= 0) ctx->filter_kind = ctx->filter_kind_request;
     else if (!ctx->anchor_enabled) ctx->filter_kind = 2 | 16;
     else if (ctx->n_kmers <= ctx->filter_group4_max) ctx->filter_kind = 2 | 4 | 16;

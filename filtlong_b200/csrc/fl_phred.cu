@@ -950,9 +950,8 @@ int fl_score_phred(fl_ctx *ctx, const BatchView &b) {
             ti.many = ctx->tie_many;
             memcpy(ti.ch, ctx->tie_char, 64);
             // (One fused pass -- a 16-byte {q, a} gather per base feeding both chains, the step one window long -- was
-            // built and measured: 14 % MORE instructions, because the sum's bookkeeping then runs once per 250 bases
-            // instead of once per 512, and 80 registers / 24 warps per SM: 31.7 ms against 23.8. Evidence:
-            // profiles/r02_ncu_c2_phred_score_fused_scale0.25.json; the code is gone.)
+            // built and measured slower: 14 % MORE instructions, because the sum's bookkeeping then runs once per 250 bases
+            // instead of once per 512, and 80 registers cost a quarter of the warps; the code is gone.)
             k_phred_sum<<<blocks, PT_THREADS, PT_SMEM, st>>>(a, ti);
             if (ws <= 64) k_phred_win<2><<<blocks, PT_THREADS, PT_SMEM, st>>>(a);
             else if (ws <= 128) k_phred_win<4><<<blocks, PT_THREADS, PT_SMEM, st>>>(a);

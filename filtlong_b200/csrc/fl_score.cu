@@ -49,10 +49,10 @@ struct ProbeArgs {
     uint32_t *mask;                          // 1 bit per padded base, same coordinates as the arena
 };
 
-// Loads of the membership tables are ld.global.nc.L1::no_allocate (no L1 line fill for a random probe). Measured and
-// dropped (profiles/): plain ld.global.nc / ld.global.cg, L2 eviction-priority hints on filter / table / mask traffic,
-// the persisting-L2 window, and .L2::64B on the table sectors (it halves the DRAM bytes, not the time: the ceiling is
-// L2-missing REQUESTS per second, profiles/r02_sector_fetch_microbench*).
+// Single-word loads of the membership tables are ld.global.nc.L1::no_allocate (no L1 line fill for a random probe).
+// Measured and dropped: ld.global.cg, L2 eviction-priority hints on filter / table / mask traffic, the persisting-L2
+// window, and .L2::64B on the table sectors (it halves the DRAM bytes, not the time: the ceiling is L2-missing
+// REQUESTS per second).
 // word holding the membership bit of `kmer`, and the bit's index, for the k-mer that starts at a read
 // position whose low two bits are pos_lo2
 template <bool ANCH>
@@ -67,7 +67,7 @@ __device__ __forceinline__ uint32_t probe(const uint32_t *__restrict__ bitmap, u
     return v;
 }
 
-// (compiled for 5 / 6 blocks per SM the pair-keyed variant spills and runs in 94 / 115 ms against 86: profiles/r02_probe_variants5_blocks_per_sm.jsonl)
+// (compiled for 5 / 6 blocks per SM the pair-keyed variant spills and runs slower)
 template <int FILT, bool ANCH>
 __global__ void __launch_bounds__(256, 4) k_probe_paint(ProbeArgs a) {
     const unsigned lane = threadIdx.x & 31;
@@ -169,7 +169,9 @@ __global__ void __launch_bounds__(256, 4) k_probe_paint(ProbeArgs a) {
                 }
                 if (ANCH) {
                     // the four 16-mers starting at 4g .. 4g+3 of the lane's run (a multiple of 32, so of 4)
-                    // share one 32-byte sector of the anchored table: ONE 256-bit load per group
+                    // share one 32-byte sector of the anchored table, read as its two 128-bit halves (sm_90 has no
+                    // 256-bit load). Lane pairs loading the two halves of one sector in one instruction and trading them
+                    // by shuffles were measured slower on an H100 (400 W): config 3 probe 137 against 116 ms, config 5 equal.
                     uint32_t sec[4][8];
 #pragma unroll
                     for (int g = 0; g < 4; ++g) {
@@ -177,10 +179,11 @@ __global__ void __launch_bounds__(256, 4) k_probe_paint(ProbeArgs a) {
                         const uint32_t key = (fl_kmer_at(w, p0 + 3) >> 6) & 0x3FFFFFFu;   // bases p0+3 .. p0+15
                         const bool need = p0 < nvalid && ((go >> (4 * g)) & 0xFu);
                         if (need) {
-                            asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                                         : "=r"(sec[g][0]), "=r"(sec[g][1]), "=r"(sec[g][2]), "=r"(sec[g][3]), "=r"(sec[g][4]),
-                                           "=r"(sec[g][5]), "=r"(sec[g][6]), "=r"(sec[g][7])
-                                         : "l"(table + (size_t)key * 8u));
+                            const uint32_t *s = table + (size_t)key * 8u;
+                            asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];"
+                                         : "=r"(sec[g][0]), "=r"(sec[g][1]), "=r"(sec[g][2]), "=r"(sec[g][3]) : "l"(s));
+                            asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];"
+                                         : "=r"(sec[g][4]), "=r"(sec[g][5]), "=r"(sec[g][6]), "=r"(sec[g][7]) : "l"(s + 4));
                         } else {
 #pragma unroll
                             for (int q = 0; q < 8; ++q) sec[g][q] = 0u;
@@ -898,7 +901,7 @@ static int score_kmer_front(fl_ctx *ctx, const BatchView &b) {
         if (blocks < 1) blocks = 1;
         {
             KernelTimer kt(ctx, FL_KERNEL_PROBE_PAINT);
-            // Measured and dropped (profiles/r02_probe_filter_experiments.md, r02_probe_variants*.jsonl): a minimizer-keyed
+            // Measured and dropped: a minimizer-keyed
             // pre-filter with per-lane load de-duplication, L2 eviction hints, the persisting-L2 window, .L2::64B table loads.
             if (ctx->use_anchor) {
                 const int filt = !ctx->use_filter ? 0 : ((ctx->filter_kind & 4) ? 2 : ((ctx->filter_kind & 8) ? 3 : 1));

@@ -97,7 +97,7 @@ const Opt kOpts[] = {
     {0, "trim", false, "trim", "trim non-k-mer-matching bases from start/end of reads"},
     {0, "split", true, "split", "split reads at this many (or more) consecutive non-k-mer-matching bases (unit suffixes: k, kb, m, mb, g, gb)"},
     {0, "window_size", true, "int", "size of sliding window used when measuring window quality (default: 250)"},
-    {0, "gpus", true, "int", "number of B200 GPUs to shard the read set across (default: 1; not a reference option)"},
+    {0, "gpus", true, "int", "number of GPUs to shard the read set across (default: 1; not a reference option)"},
     {0, "verbose", false, "verbose", "verbose output to stderr with info for each read"},
     {0, "version", false, "version", "display the program version and quit"},
     {'h', "help", false, "help", "display this help menu"},

@@ -42,7 +42,7 @@ public:
 
     int window_size = 250;
     bool verbose = false;
-    int gpus = 1;                 // B200 build only: shard the read set across this many GPUs (one context + one thread each)
+    int gpus = 1;                 // this build only: shard the read set across this many GPUs (one context + one thread each)
 
 private:
     bool does_file_exist(const std::string &filename);

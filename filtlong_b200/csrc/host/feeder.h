@@ -1,4 +1,4 @@
-// filtlong_b200/csrc/host/feeder.h -- the B200-first input path of the CLI (SURVEY 8f-1..3).
+// filtlong_b200/csrc/host/feeder.h -- the device-first input path of the CLI (SURVEY 8f-1..3).
 //
 // The reference parses its input one record at a time on one thread, twice (reference src/main.cpp:70-125 and
 // 263-313, klib kseq over zlib). Here, for an uncompressed file in the common layout (4-line FASTQ / 2-line

@@ -28,7 +28,7 @@ public:
     uint32_t base_to_bits_forward(char base);
     uint32_t base_to_bits_reverse(char base);
 
-    // additions of the B200 build
+    // additions of the CUDA build
     uint64_t size();               // m_kmers.size()
     fl_ctx *context();
     static void check(fl_ctx *ctx, int rc, const char *what);          // throws on a non-zero status

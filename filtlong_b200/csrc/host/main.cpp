@@ -1,4 +1,4 @@
-// filtlong_b200/csrc/host/main.cpp -- the `filtlong` command line on a B200.
+// filtlong_b200/csrc/host/main.cpp -- the `filtlong` command line on an H100.
 //
 // Same flow, same stderr log and same stdout as the reference's main (reference
 // src/main.cpp:37-321), restructured around batches: records are parsed and packed on the host,
@@ -66,7 +66,7 @@ int main(int argc, char **argv) {
     std::ios::sync_with_stdio(false);
     std::cerr << "\n";
     PhaseTimer timer;
-    // The CUDA driver and context take about a second to come up on a B200: start that now, on
+    // The CUDA driver and context take about a second to come up: start that now, on
     // its own thread, and parse / pack the first records meanwhile (Kmers creates its context on
     // first use). Joined on every way out of main.
     struct Warmup {
@@ -80,7 +80,7 @@ int main(int argc, char **argv) {
         const bool kmers_empty = kmers.empty();
         timer.mark("reference k-mers (+ CUDA init)");
 
-        // ---- the B200-first input path: the file as text to the device, survivors by writev from the mapping ----
+        // ---- the device-first input path: the file as text to the device, survivors by writev from the mapping ----
         {
             const FeederOutcome fo = run_text_feeder(args, kmers, [&](const char *what) { timer.mark(what); });
             if (fo.handled) return fo.exit_code;

@@ -1,4 +1,4 @@
-/* include/filtlong_b200.h -- C ABI of libfiltlong_b200.so (sm_100a CUDA inside).
+/* include/filtlong_b200.h -- C ABI of libfiltlong_b200.so (sm_90a CUDA inside).
  *
  * Drop-in boundary for Filtlong's per-read scoring / filtering hot path. Every entry point names
  * the reference interface it replaces (file:line relative to rrwick/Filtlong v0.3.1):
@@ -85,7 +85,7 @@ typedef struct fl_ctx fl_ctx;
 
 /* ---- context ------------------------------------------------------------------------------ */
 int fl_ctx_create(const fl_params *params, int device, fl_ctx **out);
-/* Optional: initialise the CUDA driver and the device's primary context (0.5-1.5 s on a B200) from
+/* Optional: initialise the CUDA driver and the device's primary context (typically 0.5-1.5 s) from
  * any thread, e.g. while the caller is still parsing its input (the reference has no counterpart:
  * its Kmers / Read constructors are ready instantly, src/main.cpp:53,108). fl_ctx_create works
  * without it. Returns FL_OK or FL_ENODEV. */

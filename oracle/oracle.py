@@ -1,13 +1,23 @@
 """oracle/oracle.py -- TEST INFRASTRUCTURE, not product code.
 
 ctypes front-end for (a) oracle/liboracle.so, our plain-C restatement of the reference path, and
-(b) oracle/_ref/refdump + oracle/_ref/filtlong_ref, the UNMODIFIED reference compiled from
-/root/reference/src by oracle/Makefile. Only tests/, __graft_entry__.smoke() and bench.py's
-cpu_baseline / --impl reference legs import this module; filtlong_b200/ never does.
+(b) oracle/_ref/refdump + oracle/_ref/filtlong_ref, the UNMODIFIED reference compiled by
+oracle/Makefile from a Filtlong v0.3.1 source tree (REF=<dir>). Only tests/, __graft_entry__.smoke()
+and bench.py's cpu_baseline / --impl reference legs import this module; filtlong_b200/ never does.
+
+Runs of (b) made by the tests are recorded in tests/golden/reference_runs.json.xz, keyed by the
+command line and the CONTENT of its input files, and replayed from there: the comparisons with the
+reference need neither its sources nor its binaries. FL_REFERENCE_RECORD=<file> runs the binaries
+instead (they must exist) and appends every run to <file>; `python -m oracle.oracle merge <file>...`
+then adds those runs to the golden store (a run recorded again replaces the stored one).
 """
 import ctypes as C
+import hashlib
+import json
+import lzma
 import os
 import subprocess
+import zlib
 from dataclasses import dataclass, field
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -17,7 +27,7 @@ REFCLI = os.path.join(HERE, "_ref", "filtlong_ref")
 
 
 def build(quiet=True):
-    """make liboracle.so (always) and _ref/ (only where /root/reference exists)."""
+    """make liboracle.so (always) and _ref/ (only where the reference sources are found, oracle/Makefile)."""
     out = subprocess.run(["make", "-C", HERE, "all"], capture_output=True, text=True)
     if out.returncode != 0:
         raise RuntimeError("oracle build failed:\n" + out.stdout + out.stderr)
@@ -239,6 +249,147 @@ def have_ref():
     return os.path.exists(REFDUMP) and os.path.exists(REFCLI)
 
 
+GOLDEN = os.path.join(os.path.dirname(HERE), "tests", "golden", "reference_runs.json.xz")
+STDOUT_INLINE = 4096          # larger stdout is kept as its SHA-256 (and, for FASTQ, the record names)
+_store = None
+
+
+def _content_digest(path):
+    """SHA-256 of what the reference reads from `path`: a gzip file by its inflated bytes (so that the
+    header's time stamp does not matter; a truncated stream by what inflates before the cut)."""
+    with open(path, "rb") as f:
+        data = f.read()
+    if data[:2] != b"\x1f\x8b":
+        return "raw:" + hashlib.sha256(data).hexdigest()
+    h, rest, ok = hashlib.sha256(), data, True
+    while rest[:2] == b"\x1f\x8b":
+        d = zlib.decompressobj(16 + zlib.MAX_WBITS)
+        try:
+            h.update(d.decompress(rest))
+        except zlib.error:
+            ok = False
+            break
+        if not d.eof:
+            ok = False
+            break
+        rest = d.unused_data
+    return ("gz:" if ok else "gz-truncated:") + h.hexdigest()
+
+
+def _file_args(args):
+    return [i for i, a in enumerate(args) if os.path.isfile(a)]
+
+
+def _key(tool, args, mode):
+    parts = [tool, mode] + [("file:" + _content_digest(a)) if os.path.isfile(a) else a for a in args]
+    return hashlib.sha256(json.dumps(parts).encode()).hexdigest()[:32]
+
+
+def _mask(text, args, files):
+    for i in sorted(files, key=lambda i: -len(args[i])):
+        text = text.replace(args[i], "{ARG%d}" % i)
+    return text
+
+
+def _unmask(text, args, files):
+    for i in files:
+        text = text.replace("{ARG%d}" % i, args[i])
+    return text
+
+
+def _load_store():
+    global _store
+    if _store is None:
+        _store = {}
+        if os.path.exists(GOLDEN):
+            with lzma.open(GOLDEN, "rt") as f:
+                _store = json.load(f)
+    return _store
+
+
+class RecordedStdout:
+    """The stdout of a recorded reference run too large to keep: equal to the bytes with its SHA-256."""
+
+    def __init__(self, sha256, size, fastq_names):
+        self.sha256, self.size, self.fastq_names = sha256, size, fastq_names
+
+    def __eq__(self, other):
+        if isinstance(other, RecordedStdout):
+            return (self.sha256, self.size) == (other.sha256, other.size)
+        if isinstance(other, (bytes, bytearray)):
+            return len(other) == self.size and hashlib.sha256(other).hexdigest() == self.sha256
+        return NotImplemented
+
+    def __len__(self):
+        return self.size
+
+    def __repr__(self):
+        return "<reference stdout: %d bytes, sha256 %s>" % (self.size, self.sha256[:16])
+
+
+def fastq_names(out):
+    """Record names of FASTQ output (bytes or RecordedStdout), None if it is not 4-line FASTQ."""
+    if isinstance(out, RecordedStdout):
+        return out.fastq_names
+    lines = out.split(b"\n")
+    if lines and lines[-1] == b"":
+        lines.pop()
+    if not lines or len(lines) % 4 or not all(l.startswith(b"@") for l in lines[0::4]):
+        return None
+    return [l[1:].split()[0].decode() for l in lines[0::4]]
+
+
+def run_reference(tool, args, env_extra=None, cwd=None, timeout=3600, kmers_out=False):
+    """One run of a reference binary ("refdump" or "filtlong_ref"): (returncode, stdout bytes, stderr str,
+    SHA-256 of the k-mer dump or None). Replayed from the golden store; FL_REFERENCE_RECORD runs and records it.
+    kmers_out: True for the dump's SHA-256, or a path to keep the dump itself (a live run only)."""
+    args = [str(a) for a in args]
+    env_extra = dict(env_extra or {})
+    mode = env_extra.get("REFDUMP_MODE", "dump") + ("+kmers" if kmers_out else "") + ("+quiet" if "REFDUMP_QUIET" in env_extra else "")
+    cwd_args = [os.path.join(cwd, a) if cwd and not os.path.isabs(a) and os.path.isfile(os.path.join(cwd, a)) else a for a in args]
+    files = _file_args(cwd_args)
+    key = _key(tool, cwd_args, mode)
+    record_to = os.environ.get("FL_REFERENCE_RECORD")
+    if not record_to:
+        if isinstance(kmers_out, str):
+            raise RuntimeError("writing the reference's k-mer dump needs a live run (FL_REFERENCE_RECORD=<file>)")
+        rec = _load_store().get(key)
+        if rec is None:
+            raise RuntimeError("no recorded reference run for %s %s (key %s): record it with FL_REFERENCE_RECORD=<file> where "
+                               "oracle/_ref is built, and merge the file into %s" % (tool, " ".join(args), key, GOLDEN))
+        out = rec["stdout"].encode("latin-1") if "stdout" in rec else RecordedStdout(rec["stdout_sha256"], rec["stdout_size"],
+                                                                                    rec.get("fastq_names"))
+        if isinstance(out, bytes):
+            out = _unmask(out.decode("latin-1"), args, files).encode("latin-1")
+        return rec["rc"], out, _unmask(rec["stderr"], args, files), rec.get("kmers_sha256")
+    kpath = None
+    if kmers_out:
+        import tempfile
+        if isinstance(kmers_out, str):
+            kpath = kmers_out
+        else:
+            fd, kpath = tempfile.mkstemp(prefix="refdump_kmers_")
+            os.close(fd)
+        env_extra["REFDUMP_KMERS_OUT"] = kpath
+    binary = {"refdump": REFDUMP, "filtlong_ref": REFCLI}[tool]
+    p = subprocess.run([binary] + args, capture_output=True, env=_env(env_extra), cwd=cwd, timeout=timeout)
+    err = p.stderr.decode(errors="replace")
+    rec = {"rc": p.returncode, "stderr": _mask(err, args, files)}
+    if len(p.stdout) <= STDOUT_INLINE or tool == "refdump":
+        rec["stdout"] = _mask(p.stdout.decode("latin-1"), args, files)
+    else:
+        rec.update(stdout_sha256=hashlib.sha256(p.stdout).hexdigest(), stdout_size=len(p.stdout), fastq_names=fastq_names(p.stdout))
+    ksha = None
+    if kpath:
+        with open(kpath, "rb") as f:
+            ksha = rec["kmers_sha256"] = hashlib.sha256(f.read()).hexdigest()
+        if kpath is not kmers_out:
+            os.unlink(kpath)
+    with open(record_to, "a") as f:
+        f.write(json.dumps({key: rec}) + "\n")
+    return p.returncode, p.stdout, err, ksha
+
+
 def _env(extra=None):
     e = dict(os.environ)
     e.pop("LANG", None)
@@ -253,19 +404,15 @@ def fromhex(s):
     return float.fromhex(s) if s not in ("nan", "-nan", "inf", "-inf") else float(s)
 
 
-def run_refdump(cli_args, kmers_out=None, quiet=False, timeout=3600):
-    """Run the link-harness over the reference objects; returns a dict of parsed records."""
-    extra = {}
-    if kmers_out:
-        extra["REFDUMP_KMERS_OUT"] = kmers_out
-    if quiet:
-        extra["REFDUMP_QUIET"] = "1"
-    out = subprocess.run([REFDUMP] + list(cli_args), capture_output=True, text=True, env=_env(extra),
-                         timeout=timeout)
-    if out.returncode != 0:
-        raise RuntimeError("refdump failed (%d): %s" % (out.returncode, out.stderr[-2000:]))
-    res = {"reads": [], "rows": [], "n_kmers": None, "global": None, "tail": None}
-    for line in out.stdout.splitlines():
+def run_refdump(cli_args, kmers_out=False, quiet=False, timeout=3600):
+    """Run the link-harness over the reference objects; returns a dict of parsed records (with kmers_out, also
+    "kmers_sha256": the SHA-256 of the sorted reference 16-mer set as raw little-endian uint32)."""
+    extra = {"REFDUMP_QUIET": "1"} if quiet else {}
+    rc, stdout, stderr, ksha = run_reference("refdump", cli_args, extra, timeout=timeout, kmers_out=kmers_out)
+    if rc != 0:
+        raise RuntimeError("refdump failed (%d): %s" % (rc, stderr[-2000:]))
+    res = {"reads": [], "rows": [], "n_kmers": None, "global": None, "tail": None, "kmers_sha256": ksha}
+    for line in stdout.decode("latin-1").splitlines():
         f = line.split(" ")
         if f[0] == "K":
             res["n_kmers"] = int(f[1])
@@ -302,10 +449,9 @@ def run_refdump_time(cli_args, timeout=3600):
 
 
 def run_refdump_bloom(keys):
-    out = subprocess.run([REFDUMP] + ["%08X" % k for k in keys], capture_output=True, text=True,
-                         env=_env({"REFDUMP_MODE": "bloom"}))
+    _, stdout, _, _ = run_reference("refdump", ["%08X" % k for k in keys], {"REFDUMP_MODE": "bloom"})
     res = {"salts": [], "hashes": {}}
-    for line in out.stdout.splitlines():
+    for line in stdout.decode("latin-1").splitlines():
         f = line.split()
         if f[0] == "BLOOM":
             res["k"], res["bits"] = int(f[1]), int(f[2])
@@ -316,7 +462,29 @@ def run_refdump_bloom(keys):
     return res
 
 
-def run_refcli(cli_args, timeout=3600):
-    """Run the unmodified reference CLI; returns (returncode, stdout, stderr)."""
-    out = subprocess.run([REFCLI] + list(cli_args), capture_output=True, text=True, env=_env(), timeout=timeout)
-    return out.returncode, out.stdout, out.stderr
+def run_refcli(cli_args, cwd=None, timeout=3600):
+    """Run the unmodified reference CLI; returns (returncode, stdout bytes or RecordedStdout, stderr str)."""
+    rc, out, err, _ = run_reference("filtlong_ref", cli_args, cwd=cwd, timeout=timeout)
+    return rc, out, err
+
+
+def merge_recorded(paths, store=GOLDEN):
+    """Adds the runs recorded under FL_REFERENCE_RECORD (JSON lines) to the golden store; returns its size."""
+    runs = {}
+    if os.path.exists(store):
+        with lzma.open(store, "rt") as f:
+            runs = json.load(f)
+    for path in paths:
+        with open(path) as f:
+            for line in f:
+                runs.update(json.loads(line))
+    with lzma.open(store, "wt", preset=9 | lzma.PRESET_EXTREME) as f:
+        json.dump(runs, f, sort_keys=True, separators=(",", ":"))
+    return len(runs)
+
+
+if __name__ == "__main__":
+    import sys
+    if len(sys.argv) < 3 or sys.argv[1] != "merge":
+        raise SystemExit("usage: python -m oracle.oracle merge <recorded runs>...")
+    print("%d reference runs in %s" % (merge_recorded(sys.argv[2:]), GOLDEN))

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generates tests/golden/*.json: outputs of the UNMODIFIED reference (oracle/_ref/refdump, i.e.
 the reference's own read.o / kmers.o) on seeded synthetic inputs, doubles as C99 hex floats.
-Run in the build container (needs /root/reference compiled by `make -C oracle`):
+Run where oracle/_ref is built (`make -C oracle REF=<Filtlong v0.3.1 source tree>`):
 
     python tests/golden/make_golden.py
 
@@ -48,7 +48,8 @@ def h(x):
 
 
 def main():
-    assert orc.have_ref(), "build oracle/_ref first (make -C oracle)"
+    assert orc.have_ref(), "build oracle/_ref first (make -C oracle REF=<Filtlong v0.3.1 source tree>)"
+    os.environ.setdefault("FL_REFERENCE_RECORD", os.devnull)      # live runs of the reference binaries
     out_dir = os.path.dirname(os.path.abspath(__file__))
     for name, case in CASES.items():
         genome_n, reads, short = inputs(case)

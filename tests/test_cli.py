@@ -1,5 +1,5 @@
 """The `filtlong` drop-in command line (filtlong_b200/bin/filtlong) against the unmodified
-reference binary (oracle/_ref/filtlong_ref): byte-identical stdout, and the stderr log lines the
+reference binary (oracle/_ref/filtlong_ref, its runs replayed from tests/golden): byte-identical stdout, and the stderr log lines the
 reference's own tests assert (test/test_sort.py, test_trim.py, test_split.py,
 test_error_messages.py, test_unit_suffixes.py). Argument errors need no GPU; everything that
 scores reads is marked gpu."""
@@ -15,7 +15,7 @@ from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CLI = os.path.join(ROOT, "filtlong_b200", "bin", "filtlong")
-need_cli = pytest.mark.skipif(not (os.path.exists(CLI) and orc.have_ref()), reason="CLI or oracle/_ref not built")
+need_cli = pytest.mark.skipif(not os.path.exists(CLI), reason="CLI not built")
 
 
 def run(binary, args, cwd=None):
@@ -69,7 +69,7 @@ def test_argument_handling_matches_reference(case, tmp_path):
     (help text only by the substrings the reference's tests check)."""
     fq = util.write_fastq(tmp_path / "x.fastq", [("r1", b"ACGT" * 10, b"I" * 40)])
     args = [fq if a == "X" else a for a in case]
-    rc_r, out_r, err_r = run(orc.REFCLI, args, cwd=tmp_path)
+    rc_r, out_r, err_r = orc.run_refcli(args, cwd=tmp_path)
     rc_o, out_o, err_o = run(CLI, args, cwd=tmp_path)
     assert rc_o == rc_r
     assert out_o == out_r
@@ -124,7 +124,7 @@ def test_cli_output_matches_reference(case, tmp_path):
     fq, fa, s1, s2, fasta_reads = make_inputs(tmp_path)
     sub = {"FQ": fq, "FA": fa, "S1": s1, "S2": s2, "FASTA": fasta_reads}
     args = [sub.get(a, a) for a in case]
-    rc_r, out_r, err_r = run(orc.REFCLI, args)
+    rc_r, out_r, err_r = orc.run_refcli(args)
     rc_o, out_o, err_o = run(CLI, args)
     assert rc_o == rc_r == 0, err_o[-2000:]
     assert out_o == out_r, "stdout differs"
@@ -145,8 +145,10 @@ def test_cli_runtime_errors_match_reference(tmp_path):
     fa = util.write_fasta(tmp_path / "reads.fasta", [("a", b"ACGT" * 30)])
     mixed = tmp_path / "mixed.fastq"
     mixed.write_bytes(b"@a\nACGTACGT\n+\nIIIIIIII\n>b\nACGTACGT\n")
-    for args in (["-t", "100", dup], ["-t", "100", str(bad)], ["-t", "100", fa], ["-t", "100", str(mixed)]):
-        rc_r, out_r, err_r = run(orc.REFCLI, args)
+    ref_bad = os.path.join(util.REF_FIXTURES, "test_bad_fastq.fastq")             # the reference suite's test_bad_fastq
+    for args in (["-t", "100", dup], ["-t", "100", str(bad)], ["-t", "100", fa], ["-t", "100", str(mixed)],
+                 ["--target_bases", "1000", ref_bad]):
+        rc_r, out_r, err_r = orc.run_refcli(args)
         rc_o, out_o, err_o = run(CLI, args)
         assert (rc_o, out_o) == (rc_r, out_r)
         assert final_lines(err_o) == final_lines(err_r)

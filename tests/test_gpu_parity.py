@@ -273,10 +273,9 @@ def test_fasta_without_reference_is_rejected():
     ctx.close()
 
 
-@pytest.mark.skipif(not orc.have_ref(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("mode", ["phred", "assembly", "short"])
 def test_against_the_real_reference_harness(mode, tmp_path):
-    """Same inputs through the UNMODIFIED reference objects (oracle/_ref/refdump) and the CUDA path."""
+    """Same inputs through the UNMODIFIED reference objects (oracle/_ref/refdump, replayed from tests/golden) and the CUDA path."""
     rng, genome, genome_n, reads = make_kmer_case(77, n_reads=120)
     named = [("r%d" % i, s, q) for i, (s, q) in enumerate(reads)]
     fq = util.write_fastq(tmp_path / "reads.fastq", named)

@@ -1,6 +1,6 @@
 """The reference-compatible C++ classes (filtlong_b200/csrc/host: Kmers, Read) used the way the
 reference's main uses them -- `Read(name, seq, qscores, length, &kmers, &args)` per record -- against
-the unmodified reference objects (oracle/_ref/refdump). Same public fields, same values."""
+the unmodified reference objects (oracle/_ref/refdump, replayed from tests/golden). Same public fields, same values."""
 import os
 import subprocess
 
@@ -12,7 +12,7 @@ from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "filtlong_b200")
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not orc.have_ref(), reason="oracle/_ref not built")]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")

@@ -1,6 +1,6 @@
 """The sharded path as the product runs it: one process per GPU, one NCCL communicator behind the C ABI
 (fl_comm_init / fl_kmers_broadcast / collective fl_finalize). Needs >= 2 GPUs (skipped otherwise):
-    gpurun --gpus 2 -- python -m pytest tests/test_nccl_ranks.py -m gpu
+    python -m pytest tests/test_nccl_ranks.py -m gpu      (on a machine with two or more GPUs)
 The union of the ranks' rows must equal what one context computes on the whole read set, and the oracle."""
 import os
 import subprocess

@@ -1,10 +1,11 @@
 """Pins oracle/filtlong_oracle.c (our C restatement) against the REAL reference.
 
-Runs on CPU. Needs oracle/_ref (the unmodified reference compiled by oracle/Makefile from
-/root/reference/src); the reference's own fixtures are read from /root/reference/test when
-present. Every double is compared bit-for-bit (the restatement follows the reference's
-operation order, so anything else is a restatement bug).
+Runs on CPU. The runs of oracle/_ref (the unmodified reference compiled by oracle/Makefile) are
+replayed from tests/golden/reference_runs.json.xz; the reference's own fixtures are the copies under
+tests/golden/ref_fixtures. Every double is compared bit-for-bit (the restatement follows the
+reference's operation order, so anything else is a restatement bug).
 """
+import hashlib
 import os
 import struct
 
@@ -13,9 +14,6 @@ import pytest
 
 from oracle import oracle as orc
 from tests import util
-
-pytestmark = pytest.mark.skipif(not orc.have_ref(), reason="oracle/_ref not built")
-
 
 def bits(x):
     return struct.pack("<d", x)
@@ -99,23 +97,23 @@ def test_bloom_closed_form():
 # --------------------------------------------------------------------------------------------
 # The reference's own fixtures (known answers of test/test_sort.py, test_trim.py, test_split.py)
 # --------------------------------------------------------------------------------------------
-need_fixtures = pytest.mark.skipif(not util.have_ref_fixtures(), reason="/root/reference/test absent")
-T = util.REF_TEST_DIR
+T = util.REF_FIXTURES
 
 
-@need_fixtures
+# the first 1500 pairs of the reference's test_reference_{1,2}.fastq.gz (all 20,000 are too large to store)
+S1, S2 = T + "/test_reference_1_first1500.fastq.gz", T + "/test_reference_2_first1500.fastq.gz"
+
+
 def test_kmer_counts_match_reference_log_lines():
-    # SURVEY section 4 KATs: 199,964 16-mers from the assembly; 204,833 from the short reads
+    # SURVEY section 4 KAT: 199,964 16-mers from the assembly; 23,368 from the stored short-read sample (the
+    # reference's log line on exactly these files; 204,833 on all 20,000 pairs)
     asm = util.read_fastx(T + "/test_reference.fasta")
     k = oracle_kmers(assembly=asm)
     assert len(k) == 199964
-    s1 = util.read_fastx(T + "/test_reference_1.fastq.gz")
-    s2 = util.read_fastx(T + "/test_reference_2.fastq.gz")
-    k2 = oracle_kmers(short=[s1, s2])
-    assert len(k2) == 204833
+    k2 = oracle_kmers(short=[util.read_fastx(S1), util.read_fastx(S2)])
+    assert len(k2) == 23368
 
 
-@need_fixtures
 @pytest.mark.parametrize("mode", ["phred", "assembly", "short"])
 @pytest.mark.parametrize("opts", [
     dict(min_length=1, keep_percent=90.0),           # BASELINE config 1
@@ -134,9 +132,8 @@ def test_sort_fixture(mode, opts, tmp_path):
         cli += ["-a", T + "/test_reference.fasta"]
         kmers = oracle_kmers(assembly=util.read_fastx(T + "/test_reference.fasta"))
     elif mode == "short":
-        cli += ["-1", T + "/test_reference_1.fastq.gz", "-2", T + "/test_reference_2.fastq.gz"]
-        kmers = oracle_kmers(short=[util.read_fastx(T + "/test_reference_1.fastq.gz"),
-                                    util.read_fastx(T + "/test_reference_2.fastq.gz")])
+        cli += ["-1", S1, "-2", S2]
+        kmers = oracle_kmers(short=[util.read_fastx(S1), util.read_fastx(S2)])
     ref = orc.run_refdump(cli + [T + "/test_sort.fastq"])
     sc = orc.finalize(orc.score([(r[1], r[2]) for r in reads], p, kmers), p)
     if kmers is not None:
@@ -146,7 +143,6 @@ def test_sort_fixture(mode, opts, tmp_path):
         assert (sc.summary.target, sc.summary.keeping) == (13500, 15000)
 
 
-@need_fixtures
 @pytest.mark.parametrize("fixture,opts", [
     ("test_trim.fastq", dict(trim=True)),
     ("test_trim.fastq", dict(trim=True, split=20)),
@@ -168,7 +164,6 @@ def test_trim_split_fixtures(fixture, opts, tmp_path):
     compare(ref, sc, p)
 
 
-@need_fixtures
 def test_window_drift_golden():
     """SURVEY section 4: window quality 79.999999999999986 (not 80) for test_split_2 under -a."""
     p = orc.make_params(min_length=1)
@@ -234,10 +229,9 @@ def test_random_kmer(seed, opts, use_short, tmp_path):
                                                       ("tiny", b"ACGT")], width=70)
         cli += ["-a", fa]
         kmers = oracle_kmers(assembly=[("c1", genome_n[:30000]), ("c2", genome_n[30000:])])
-    kout = str(tmp_path / "kmers.bin")
-    ref = orc.run_refdump(cli + [fq], kmers_out=kout)
+    ref = orc.run_refdump(cli + [fq], kmers_out=True)
     assert ref["n_kmers"] == len(kmers)
-    assert np.array_equal(np.fromfile(kout, dtype=np.uint32), kmers.dump())
+    assert ref["kmers_sha256"] == hashlib.sha256(kmers.dump().astype("<u4").tobytes()).hexdigest()
     sc = orc.finalize(orc.score([(r[1], r[2]) for r in reads], p, kmers), p)
     compare(ref, sc, p)
 
@@ -253,7 +247,7 @@ def test_harness_selection_matches_reference_cli(tmp_path):
         ref = orc.run_refdump(extra + [fq])
         rc, out, err = orc.run_refcli(extra + [fq])
         assert rc == 0
-        cli_names = [l[1:].split()[0] for l in out.splitlines()[0::4]]
+        cli_names = orc.fastq_names(out)
         # reads2 rows in file order; child rows carry the child name
         kept = [r["name"] for r in ref["rows"] if r["passed_final"]]
         assert cli_names == kept

@@ -1,42 +1,12 @@
-"""The reference's own black-box suite (test/test_sort.py, test_trim.py, test_split.py,
-test_error_messages.py, test_unit_suffixes.py: 93 unittest cases) run UNMODIFIED against
-filtlong_b200/bin/filtlong -- the suite finds its binary at <root>/bin/filtlong, so the staged copy under
-oracle/_ref/reftests/ (made by oracle/Makefile; expected numbers have their thousands separators stripped
-because the image has no en_US locale, nothing else) gets a bin/ that points at ours. Plus BASELINE
-config 1 and the reference's known answers on the committed fixture bytes, through the C ABI."""
+"""BASELINE config 1 and the known answers of the reference's own test suite (test/test_sort.py,
+test_trim.py, test_split.py) on the committed fixture bytes, through the C ABI."""
 import os
-import re
-import subprocess
-import sys
 
-import numpy as np
 import pytest
 
 from tests import util
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-STAGE = os.path.join(ROOT, "oracle", "_ref", "reftests")
-OURS = os.path.join(ROOT, "filtlong_b200", "bin", "filtlong")
-FIX = os.path.join(ROOT, "tests", "golden", "ref_fixtures")
-
-
-@pytest.mark.gpu
-def test_reference_unittest_suite_passes_against_our_binary():
-    assert os.path.isdir(os.path.join(STAGE, "test")), "oracle/_ref/reftests missing: run `make -C oracle` where /root/reference exists"
-    assert os.path.exists(OURS), "filtlong_b200/bin/filtlong not built"
-    link = os.path.join(STAGE, "bin", "filtlong")
-    os.makedirs(os.path.dirname(link), exist_ok=True)
-    if os.path.lexists(link):
-        os.unlink(link)
-    os.symlink(OURS, link)
-    env = dict(os.environ, LC_ALL="C")
-    env.pop("LANG", None)
-    r = subprocess.run([sys.executable, "-m", "unittest", "discover", "-s", "test", "-p", "test_*.py"], cwd=STAGE, env=env,
-                       capture_output=True, text=True, timeout=3000)
-    tail = r.stderr[-3000:]
-    m = re.search(r"Ran (\d+) tests", r.stderr)
-    assert m and int(m.group(1)) == 93, tail
-    assert r.returncode == 0 and "OK" in r.stderr.splitlines()[-1], tail
+FIX = util.REF_FIXTURES
 
 
 def _fixture_reads(name):

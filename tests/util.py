@@ -107,11 +107,7 @@ def write_fasta(path, reads, width=0):
     return str(path)
 
 
-REF_TEST_DIR = "/root/reference/test"
-
-
-def have_ref_fixtures():
-    return os.path.isdir(REF_TEST_DIR)
+REF_FIXTURES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_fixtures")
 
 
 def read_fastx(path):

@@ -4,7 +4,7 @@ binary (oracle/_ref/filtlong_ref, CPU) on the same synthetic FASTQ, same argumen
 Checks that stdout is byte-identical and reports wall-clock seconds and Gbases/s of the whole process
 (CUDA start-up included). Test / measurement infrastructure (it executes oracle/_ref); writes one JSON line.
 
-    python tools/cli_e2e.py [--small-gbp 0.5] [--large-gbp 5] [--kmer-gbp 0.1] [--gpus N] > gpurun_out/cli_e2e.json
+    python tools/cli_e2e.py [--small-gbp 0.5] [--large-gbp 5] [--kmer-gbp 0.1] [--gpus N] > cli_e2e.json
 
 Cases: a small Phred file and a k-mer + --trim --split 500 file through BOTH binaries (byte-identical stdout
 required), and a large plain FASTQ through ours only (the reference needs ~26 s per Gbp), once with the device

@@ -5,7 +5,7 @@ streaming host reader (FL_GZ_HOST=1: gzread under a kseq-compatible parser, twic
 comparison. Reports wall-clock seconds of the whole process and checks that every variant prints the same bytes.
 Measurement infrastructure; writes one JSON line.
 
-    python tools/cli_gz.py [--gbp 1.0] > gpurun_out/cli_gz.json
+    python tools/cli_gz.py [--gbp 1.0] > cli_gz.json
 """
 import argparse
 import hashlib
