@@ -240,6 +240,25 @@ class Context:
         self._ck(self.L.fl_results_reads(self.h, C.byref(o)), "fl_results_reads")
         return {k: v[:n] for k, v in r.items()}
 
+    # ---- BGZF output (fl_bgzf_compress*) ----
+    def bgzf_compress(self, data, append_eof=True):
+        """data (bytes-like) compressed as BGZF on the device: bytes that any gzip reader inflates back to data."""
+        src = np.frombuffer(data, dtype=np.uint8)
+        out = np.empty(int(self.L.fl_bgzf_bound(src.size)), dtype=np.uint8)
+        n = C.c_uint64()
+        self._ck(self.L.fl_bgzf_compress(self.h, capi.ptr(src), src.size, capi.ptr(out), out.size, int(append_eof), C.byref(n)),
+                 "fl_bgzf_compress")
+        return out[:n.value].tobytes()
+
+    def bgzf_compress_device(self, dev_in, n, dev_out, cap, append_eof=True):
+        """Device buffers (torch tensors or raw pointers); returns the compressed size, or None when cap is too small."""
+        m = C.c_uint64()
+        rc = self.L.fl_bgzf_compress_device(self.h, capi.ptr(dev_in), n, capi.ptr(dev_out), cap, int(append_eof), C.byref(m))
+        if rc == capi.FL_ERANGE:
+            return None
+        self._ck(rc, "fl_bgzf_compress_device")
+        return m.value
+
     def row_results(self):
         _, n, _ = self.counts()
         m = max(n, 1)
@@ -250,6 +269,12 @@ class Context:
         o = capi.RowResults(**{k: capi.ptr(v) for k, v in r.items()})
         self._ck(self.L.fl_results_rows(self.h, C.byref(o)), "fl_results_rows")
         return {k: v[:n] for k, v in r.items()}
+
+
+def bgzf_compress(data, append_eof=True, device=0):
+    """One-shot BGZF compression of host bytes on a fresh context (what `filtlong --bgzip` does to its output)."""
+    with Context(device=device) as ctx:
+        return ctx.bgzf_compress(data, append_eof)
 
 
 def score_and_filter(reads, params, assembly=None, short_reads=None, device=0):

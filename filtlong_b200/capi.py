@@ -13,6 +13,8 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(PKG, "libfiltlong_b200.so")
 
 FL_ALIGN_BASES = 64
+FL_BGZF_BLOCK = 65280
+FL_ERANGE = -5
 
 
 class FLError(RuntimeError):
@@ -174,6 +176,9 @@ SYMBOLS = [
     ("fl_synth_assembly_host", None, [C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint32, _P, _P]),
     ("fl_synth_ascii_device", C.c_int, [_P, C.c_uint32, _P, _P, _P, _P, _P]),
     ("fl_synth_ascii_host", None, [C.c_uint32, _P, _P, _P, _P, _P]),
+    ("fl_bgzf_bound", C.c_uint64, [C.c_uint64]),
+    ("fl_bgzf_compress", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
+    ("fl_bgzf_compress_device", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
     ("fl_version", C.c_char_p, []),
     ("fl_phred_luts", None, [C.c_int32, _P, _P]),
 ]

@@ -226,6 +226,14 @@ struct fl_ctx {
     uint64_t collectives = 0;            // NCCL calls issued so far
     bool select_attr_set = false;
 
+    // ---- BGZF compression (fl_bgzf.cu): its own buffers, so that it never touches the scored reads ----
+    DevVec<uint8_t> bz_slots;                  // one 64 KiB member slot per block of a launch
+    DevVec<uint32_t> bz_sizes;                 // member sizes of a launch
+    DevVec<unsigned long long> bz_offs;        // their output offsets
+    DevVec<unsigned long long> bz_state;       // [0] bytes written so far, [1] the output buffer was too small
+    DevVec<uint8_t> bz_hin, bz_hout;           // fl_bgzf_compress: the host buffers' device copies
+    bool bgzf_attr_set = false;
+
     // ---- optional per-kernel timing (fl_ctx_enable_timing) ----
     bool timing = false;
     struct TimedLaunch { cudaEvent_t a, b; int which; };

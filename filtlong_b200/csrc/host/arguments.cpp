@@ -98,6 +98,7 @@ const Opt kOpts[] = {
     {0, "split", true, "split", "split reads at this many (or more) consecutive non-k-mer-matching bases (unit suffixes: k, kb, m, mb, g, gb)"},
     {0, "window_size", true, "int", "size of sliding window used when measuring window quality (default: 250)"},
     {0, "gpus", true, "int", "number of GPUs to shard the read set across (default: 1; not a reference option)"},
+    {0, "bgzip", false, "bgzip", "compress the output as BGZF (gzip-compatible) on the GPU (not a reference option)"},
     {0, "verbose", false, "verbose", "verbose output to stderr with info for each read"},
     {0, "version", false, "version", "display the program version and quit"},
     {'h', "help", false, "help", "display this help menu"},
@@ -114,7 +115,7 @@ void print_help(const char *prog) {
         {"external references (if provided, read quality will be determined using these instead of from the Phred scores):", 6, 8},
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
         {"read manipulation:", 12, 13},
-        {"other:", 14, 18},
+        {"other:", 14, 19},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -158,6 +159,7 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "split") { split = read_int_suffix(nm, v); split_set = true; }
         else if (ln == "window_size") window_ll = read_plain_ll(nm, v);
         else if (ln == "gpus") gpus = (int)read_plain_ll(nm, v);
+        else if (ln == "bgzip") bgzip = true;
         else if (ln == "verbose") verbose = true;
         else if (ln == "version") version_flag = true;
         else if (ln == "help") throw HelpRequested();

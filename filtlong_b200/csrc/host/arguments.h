@@ -43,6 +43,7 @@ public:
     int window_size = 250;
     bool verbose = false;
     int gpus = 1;                 // this build only: shard the read set across this many GPUs (one context + one thread each)
+    bool bgzip = false;           // this build only: stdout compressed as BGZF on the GPU (bgzf_out.h)
 
 private:
     bool does_file_exist(const std::string &filename);

@@ -1,0 +1,58 @@
+// filtlong_b200/csrc/host/bgzf_out.h -- `--bgzip`: the CLI's output compressed as BGZF on the GPU.
+//
+// The reference prints plain FASTQ / FASTA and its README pipes it through `gzip`. BgzfOut is an output sink with the
+// interface of the CLI's other sinks (put / put_owned): the bytes are copied into pinned batches of whole 65,280-byte
+// blocks, each batch is compressed by fl_bgzf_compress and the members are written to the descriptor in order. Filling
+// the next batch (the caller's thread), compressing one (a compressor thread) and writing the one before (a writer
+// thread) overlap. finish() writes the last batch and the EOF member. The context must not be used by anyone else
+// until finish() returns.
+#pragma once
+#include <condition_variable>
+#include <cstddef>
+#include <cstdint>
+#include <deque>
+#include <mutex>
+#include <string>
+#include <thread>
+
+#include "../../../include/filtlong_b200.h"
+
+class BgzfOut {
+public:
+    BgzfOut(fl_ctx *ctx, int fd);
+    ~BgzfOut();                        // without finish(): stops the threads, writes no EOF member
+    BgzfOut(const BgzfOut &) = delete;
+    BgzfOut &operator=(const BgzfOut &) = delete;
+
+    void put(const void *p, size_t n);
+    void put_owned(std::string s) { put(s.data(), s.size()); }
+    // Compresses and writes what is left, then the EOF member. False if a compression or a write failed.
+    bool finish();
+    // why a compression failed (empty when it was a write that failed)
+    const std::string &error() const { return error_; }
+
+private:
+    static constexpr int NIN = 3, NOUT = 2;
+    void submit();
+    void compress_loop();
+    void write_loop();
+    void stop();
+    void fail(const std::string &why);
+
+    fl_ctx *ctx_;
+    int fd_;
+    uint64_t in_cap_ = 0, out_cap_ = 0;
+    char *in_[NIN] = {nullptr, nullptr, nullptr};
+    uint64_t in_len_[NIN] = {0, 0, 0};
+    bool in_busy_[NIN] = {false, false, false};
+    char *out_[NOUT] = {nullptr, nullptr};
+    uint64_t out_len_[NOUT] = {0, 0};
+    bool out_busy_[NOUT] = {false, false};
+    int fill_ = 0, next_out_ = 0;
+    std::deque<int> to_compress_, to_write_;
+    bool closing_ = false, compress_done_ = false, failed_ = false, finished_ = false;
+    std::string error_;
+    std::mutex m_;
+    std::condition_variable cv_;
+    std::thread compressor_, writer_;
+};

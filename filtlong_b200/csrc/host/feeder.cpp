@@ -20,6 +20,7 @@
 #include <thread>
 #include <vector>
 
+#include "bgzf_out.h"
 #include "misc.h"
 #include "read.h"
 #include "textsrc.h"
@@ -455,7 +456,7 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
     bool out_failed = false;
     struct stat ost;
     const int oflags = fcntl(g_out_fd, F_GETFL);
-    const bool to_file = fstat(g_out_fd, &ost) == 0 && S_ISREG(ost.st_mode) && oflags >= 0 && !(oflags & O_APPEND) && !getenv("FL_SERIAL_OUTPUT");
+    const bool to_file = !args.bgzip && fstat(g_out_fd, &ost) == 0 && S_ISREG(ost.st_mode) && oflags >= 0 && !(oflags & O_APPEND) && !getenv("FL_SERIAL_OUTPUT");
     if (to_file) {
         // stdout is a regular file: contiguous groups of reads are sized, then written with pwrite() by a few threads
         struct Sizer {
@@ -515,6 +516,13 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
         for (auto &G : groups) { G.at = total_out; total_out += G.bytes; }
         if (base_pos < 0 || !work(true)) out_failed = true;
         else if (lseek(g_out_fd, base_pos + (off_t)total_out, SEEK_SET) < 0) out_failed = true;
+    } else if (args.bgzip) {
+        // compressed offsets are not known in advance: pipe or file, the members are written in order (GPU 0 compresses)
+        BgzfOut z(ctx0, g_out_fd);
+        for (auto &s : shards)
+            for (size_t i = 0; i < s.rec.n; ++i) emit_read(z, s, i);
+        out_failed = !z.finish();
+        if (out_failed && !z.error().empty()) std::cerr << "Error: " << z.error() << "\n";
     } else {
         Writer w;
         for (auto &s : shards)

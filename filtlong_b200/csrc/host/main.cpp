@@ -16,6 +16,7 @@
 #include <cstdlib>
 #include <iostream>
 #include <limits>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <thread>
@@ -23,6 +24,7 @@
 #include <vector>
 
 #include "arguments.h"
+#include "bgzf_out.h"
 #include "fastx.h"
 #include "feeder.h"
 #include "kmers.h"
@@ -212,6 +214,12 @@ int main(int argc, char **argv) {
 
         // ---- pass 2: output the keepers in input order (main.cpp:263-313) ----
         std::cerr << "Outputting passed long reads\n";
+        std::unique_ptr<BgzfOut> zout;                                    // --bgzip: compressed on the scoring context's GPU
+        if (args.bgzip) zout.reset(new BgzfOut(kmers.context(), 1));
+        auto write_out = [&](const std::string &o) {
+            if (zout) zout->put(o.data(), o.size());
+            else fwrite(o.data(), 1, o.size(), stdout);
+        };
         bool printed = false;
         if (slices_ok && rec_seq_off.size() == reads.n_reads() && reads.n_reads() > 0) {
             // same bytes as the loop below, taken from the mapped input at the offsets pass 1 recorded
@@ -253,9 +261,9 @@ int main(int argc, char **argv) {
                                     emit(i, reads.row_name(row), start, length);
                                 }
                             }
-                            if (out.size() >= (1 << 20)) { fwrite(out.data(), 1, out.size(), stdout); out.clear(); }
+                            if (out.size() >= (1 << 20)) { write_out(out); out.clear(); }
                         }
-                        fwrite(out.data(), 1, out.size(), stdout);
+                        write_out(out);
                         fflush(stdout);
                         printed = true;
                     }
@@ -296,11 +304,15 @@ int main(int argc, char **argv) {
                         if (fastq_output) { out += "+\n"; out.append(in.qual, (size_t)start, (size_t)length); out += '\n'; }
                     }
                 }
-                if (out.size() >= (1 << 20)) { fwrite(out.data(), 1, out.size(), stdout); out.clear(); }
+                if (out.size() >= (1 << 20)) { write_out(out); out.clear(); }
                 ++i;
             }
-            fwrite(out.data(), 1, out.size(), stdout);
+            write_out(out);
             fflush(stdout);
+        }
+        if (zout && !zout->finish()) {
+            if (!zout->error().empty()) std::cerr << "Error: " << zout->error() << "\n";
+            return 1;
         }
         timer.mark("pass 2 (parse, print)");
         std::cerr << "\n";

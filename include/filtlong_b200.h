@@ -362,6 +362,25 @@ int fl_synth_ascii_device(fl_ctx *ctx, uint32_t n, const uint64_t *dev_off, cons
 void fl_synth_ascii_host(uint32_t n, const uint64_t *off, const int32_t *len, const uint32_t *seq2b,
                          const uint32_t *nmask, uint8_t *ascii);
 
+/* ---- BGZF output (no reference counterpart: replaces the `| gzip > output.fastq.gz` pipe the reference README ends
+ * its command lines with) ----------------------------------------------------------------------------------------------
+ * The input is cut into blocks of FL_BGZF_BLOCK bytes (bgzip's block size; the last one may be shorter) and every
+ * block becomes one BGZF member (SAM specification 4.1): a gzip member with MTIME 0, XFL 0, OS 255 and a 6-byte 'BC'
+ * extra field holding the member size - 1, a raw deflate stream (one dynamic-Huffman block, or a stored block when that
+ * is not larger) and the CRC-32 / ISIZE trailer. The members follow each other in input order, then, with append_eof,
+ * the 28-byte empty member that ends a BGZF file. Any gzip reader reads the result; the same input always gives the
+ * same bytes. Works on any context (one without reads or k-mers too) and leaves its scored reads and results as they
+ * are. FL_ERANGE: cap is too small; *n_out then holds the size needed. */
+#define FL_BGZF_BLOCK 65280u
+/* Largest output n_bytes of input can give, the EOF member included. */
+uint64_t fl_bgzf_bound(uint64_t n_bytes);
+/* Host buffers (pinned ones copy fastest). */
+int fl_bgzf_compress(fl_ctx *ctx, const void *host_in, uint64_t n, void *host_out, uint64_t cap, int append_eof,
+                     uint64_t *n_out);
+/* Device buffers on the context's device. */
+int fl_bgzf_compress_device(fl_ctx *ctx, const void *dev_in, uint64_t n, void *dev_out, uint64_t cap, int append_eof,
+                            uint64_t *n_out);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char *fl_version(void);
 /* Phred look-up tables exactly as the device uses them (read.cpp:270-273 evaluated with the host
