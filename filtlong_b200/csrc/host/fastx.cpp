@@ -73,6 +73,7 @@ int64_t FastxReader::next() {
     qual.clear();
     // name: up to the first whitespace character
     name.clear();
+    name_off = pos();
     bool got = false;
     for (;;) {
         c = getc();

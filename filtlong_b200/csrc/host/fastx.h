@@ -33,9 +33,9 @@ public:
     // slices of the input instead of parsing it a second time (main.cpp:263-313 re-reads the file).
     // Valid after next() >= 0. `simple` says the sequence and the quality each came from exactly one
     // line with nothing stripped, i.e. input[seq_off, seq_off + length) IS the sequence (and likewise
-    // for the quality and the comment); otherwise the offsets must not be used.
+    // for the name, the quality and the comment); otherwise the offsets must not be used.
     bool simple = false;
-    uint64_t comment_off = 0, seq_off = 0, qual_off = 0;
+    uint64_t name_off = 0, comment_off = 0, seq_off = 0, qual_off = 0;
     // true when the file is not compressed: stream offsets are file offsets
     bool plain() const { return fp_ && gzdirect(fp_) != 0; }
 

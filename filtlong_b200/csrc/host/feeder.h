@@ -10,7 +10,7 @@
 //     are compared byte for byte, in the mapping, only when two hashes agree; no string is ever built;
 //   * with --gpus N the chunks are dealt to N contexts as contiguous ranges (one thread + one NCCL rank per
 //     GPU, the 16-mer set broadcast from GPU 0, fl_finalize collective): the output is what one GPU prints;
-//   * pass 2 writes the survivors with writev() straight from the mapping (no second parse, no copies).
+//   * pass 2 writes the survivors straight from the mapping (survivors.h: writev, or pwrite groups into a regular file).
 //   * a gzip file is inflated ONCE into memory (gzmem.h: BGZF blocks by several host threads, anything else by one)
 //     and then goes down the same path; the reference inflates it once per pass.
 // Anything else -- CR LF, multi-line records, broken records, a gzip file that is damaged or would not fit in memory,

@@ -1,0 +1,255 @@
+// filtlong_b200/csrc/host/survivors.cpp -- see survivors.h.
+#include "survivors.h"
+
+#include <fcntl.h>
+#include <sys/stat.h>
+#include <sys/uio.h>
+#include <unistd.h>
+
+#include <algorithm>
+#include <atomic>
+#include <cstdio>
+#include <iostream>
+#include <thread>
+
+#include "bgzf_out.h"
+#include "fastx.h"
+#include "misc.h"
+
+bool Records::within(uint64_t file_size, bool quality) const {
+    for (size_t i = 0; i < n; ++i) {
+        const uint64_t L = (uint64_t)len[i];
+        if (name_off[i] + name_len[i] + 1 + comment_len[i] > file_size || seq_off[i] + L > file_size ||
+            (quality && qual_off[i] + L > file_size))
+            return false;
+    }
+    return true;
+}
+
+namespace {
+
+struct RecordText {               // one input record's bytes
+    const char *name;
+    size_t name_len;
+    const char *comment;
+    size_t comment_len;
+    const char *seq, *qual;
+    size_t len;
+    bool lead_before_name;        // name[-1] is the format's lead character
+};
+
+RecordText text_of(const Records &R, const char *base, size_t i) {
+    const char *name = base + R.name_off[i];
+    return RecordText{name, R.name_len[i], name + R.name_len[i] + 1, R.comment_len[i], base + R.seq_off[i], base + R.qual_off[i],
+                      (size_t)R.len[i], R.lead_checked};
+}
+
+// Read i's output: the read if it survived and has no children, else each surviving child longer than 0. put()'s bytes
+// must stay valid until the sink is flushed; put_owned() keeps its string alive until then.
+template <class Sink>
+void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Results &res, size_t i) {
+    const char *lead = fmt.lead == '>' ? ">" : "@";
+    auto rest = [&](size_t start, size_t length) {
+        if (r.comment_len) { sink.put(" ", 1); sink.put(r.comment, r.comment_len); }
+        sink.put("\n", 1);
+        sink.put(r.seq + start, length);
+        sink.put("\n", 1);
+        if (fmt.quality) { sink.put("+\n", 2); sink.put(r.qual + start, length); sink.put("\n", 1); }
+    };
+    const size_t rs = (size_t)res.row_start[i];
+    if (res.n_child[i] == 0) {
+        if (!res.row_pfinal[rs]) return;
+        if (r.lead_before_name) sink.put(r.name - 1, 1 + r.name_len);
+        else { sink.put(lead, 1); sink.put(r.name, r.name_len); }
+        rest(0, r.len);
+        return;
+    }
+    for (size_t row = rs; row < rs + (size_t)res.n_child[i]; ++row) {
+        const int start = res.row_s[row], end = res.row_e[row];
+        // (a row past the record's end can only come from an input that changed since pass 1)
+        if (!res.row_pfinal[row] || end - start <= 0 || (size_t)end > r.len) continue;
+        std::string nm(lead, 1);
+        append_child_name(nm, r.name, r.name_len, start, end);
+        sink.put_owned(std::move(nm));
+        rest((size_t)start, (size_t)(end - start));
+    }
+}
+
+template <class Sink>
+void emit_range(Sink &sink, const char *base, const Part &p, size_t lo, size_t hi, const Format &fmt) {
+    for (size_t i = lo; i < hi; ++i) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i);
+}
+
+// iovecs into the mapping, written with writev()
+struct Writer {
+    static constexpr int MAXV = 1000;
+    int fd;
+    struct iovec v[MAXV];
+    int nv = 0;
+    std::vector<std::string> small;            // child names: must stay alive (and in place: short strings live inside the object) until the flush
+    bool failed = false;
+    explicit Writer(int f) : fd(f) { small.reserve(256); }
+    void flush() {
+        int done = 0;
+        while (done < nv && !failed) {
+            ssize_t w = writev(fd, v + done, nv - done);
+            if (w < 0) { failed = true; break; }
+            while (done < nv && (size_t)w >= v[done].iov_len) { w -= (ssize_t)v[done].iov_len; ++done; }
+            if (done < nv && w > 0) { v[done].iov_base = (char *)v[done].iov_base + w; v[done].iov_len -= (size_t)w; }
+        }
+        nv = 0;
+        small.clear();
+    }
+    void put(const void *p, size_t n) {
+        if (n == 0) return;
+        if (nv == MAXV) flush();
+        v[nv].iov_base = const_cast<void *>(p);
+        v[nv].iov_len = n;
+        ++nv;
+    }
+    void put_owned(std::string s) {
+        if (nv == MAXV || small.size() >= 200) flush();
+        small.push_back(std::move(s));
+        put(small.back().data(), small.back().size());
+    }
+};
+
+struct Sizer {
+    uint64_t n = 0;
+    void put(const void *, size_t k) { n += k; }
+    void put_owned(std::string s) { n += s.size(); }
+};
+
+// copies into a buffer of about 8 MiB; flush() writes it with pwrite() at `pos`, or with write() when pos < 0
+struct Copier {
+    int fd;
+    int64_t pos;
+    std::string buf;
+    bool failed = false;
+    Copier(int f, int64_t p) : fd(f), pos(p) { buf.reserve((8u << 20) + (2u << 20)); }
+    void flush() {
+        size_t done = 0;
+        while (done < buf.size() && !failed) {
+            const ssize_t w = pos < 0 ? write(fd, buf.data() + done, buf.size() - done)
+                                      : pwrite(fd, buf.data() + done, buf.size() - done, (off_t)(pos + (int64_t)done));
+            if (w <= 0) { failed = true; break; }
+            done += (size_t)w;
+        }
+        if (pos >= 0) pos += (int64_t)buf.size();
+        buf.clear();
+    }
+    void put(const void *p, size_t k) { buf.append((const char *)p, k); if (buf.size() >= (8u << 20)) flush(); }
+    void put_owned(std::string s) { put(s.data(), s.size()); }
+};
+
+bool finish(BgzfOut &z) {
+    if (z.finish()) return true;
+    if (!z.error().empty()) std::cerr << "Error: " << z.error() << "\n";
+    return false;
+}
+
+}  // namespace
+
+bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt) {
+    Writer w(fd);
+    for (const Part &p : parts) emit_range(w, base, p, 0, p.rec->n, fmt);
+    w.flush();
+    return !w.failed;
+}
+
+// contiguous groups of reads are sized, then written with pwrite() by a few threads
+bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt) {
+    struct Group { size_t part, lo, hi; uint64_t bytes = 0, at = 0; };
+    std::vector<Group> groups;
+    size_t n_reads = 0;
+    for (const Part &p : parts) n_reads += p.rec->n;
+    const size_t per = n_reads / 32 + 1;
+    for (size_t pi = 0; pi < parts.size(); ++pi)
+        for (size_t lo = 0; lo < parts[pi].rec->n; lo += per) groups.push_back(Group{pi, lo, std::min(lo + per, parts[pi].rec->n), 0, 0});
+    const off_t base_pos = lseek(fd, 0, SEEK_CUR);
+    auto work = [&](bool write_pass) {
+        std::vector<std::thread> ts;
+        std::atomic<size_t> next(0);
+        std::atomic<bool> bad(false);
+        const unsigned nt = std::min<size_t>(8, groups.size());
+        for (unsigned t = 0; t < nt; ++t)
+            ts.emplace_back([&] {
+                for (size_t g = next.fetch_add(1); g < groups.size(); g = next.fetch_add(1)) {
+                    Group &G = groups[g];
+                    if (!write_pass) {
+                        Sizer z;
+                        emit_range(z, base, parts[G.part], G.lo, G.hi, fmt);
+                        G.bytes = z.n;
+                    } else {
+                        Copier c(fd, (int64_t)base_pos + (int64_t)G.at);
+                        emit_range(c, base, parts[G.part], G.lo, G.hi, fmt);
+                        c.flush();
+                        if (c.failed) bad.store(true);
+                    }
+                }
+            });
+        for (auto &t : ts) t.join();
+        return !bad.load();
+    };
+    work(false);
+    uint64_t total_out = 0;
+    for (auto &G : groups) { G.at = total_out; total_out += G.bytes; }
+    if (base_pos < 0 || !work(true)) return false;
+    return lseek(fd, base_pos + (off_t)total_out, SEEK_SET) >= 0;
+}
+
+bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf) {
+    fflush(stdout);
+    if (bgzf) {
+        // compressed offsets are not known in advance: pipe or file, the members are written in order
+        BgzfOut z(bgzf, fd);
+        for (const Part &p : parts) emit_range(z, base, p, 0, p.rec->n, fmt);
+        return finish(z);
+    }
+    struct stat st;
+    const int flags = fcntl(fd, F_GETFL);
+    if (fstat(fd, &st) == 0 && S_ISREG(st.st_mode) && flags >= 0 && !(flags & O_APPEND))
+        return write_survivors_pwrite(fd, base, parts, fmt);
+    return write_survivors_writev(fd, base, parts, fmt);
+}
+
+bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+    fflush(stdout);
+    FastxReader in(path);
+    auto run = [&](auto &sink) {
+        for (size_t i = 0; in.ok() && in.next() >= 0 && i < n_reads; ++i) {
+            const RecordText r{in.name.data(), in.name.size(), in.comment.data(), in.comment.size(), in.seq.data(), in.qual.data(),
+                               in.seq.size(), false};
+            emit_survivors(sink, fmt, r, res, i);
+        }
+    };
+    if (bgzf) {
+        BgzfOut z(bgzf, fd);
+        run(z);
+        return finish(z);
+    }
+    Copier c(fd, -1);
+    run(c);
+    c.flush();
+    return !c.failed;
+}
+
+void log_after_trim_split(const Arguments &args, uint64_t n_rows, const fl_summary &summary) {
+    if (args.trim || args.split_set) {
+        if (args.trim && args.split_set) std::cerr << "  after trimming and splitting: ";
+        else if (args.trim) std::cerr << "  after trimming: ";
+        else std::cerr << "  after splitting: ";
+        std::cerr << int_to_string((long long)n_rows) << " reads (" << int_to_string(summary.rows_bases) << " bp)\n";
+    }
+    std::cerr << "\n";
+}
+
+void log_filtering(const Arguments &args, const fl_summary &summary) {
+    if (!args.target_bases_set && !args.keep_percent_set) return;
+    std::cerr << "Filtering long reads\n";
+    std::cerr << "  target: " << int_to_string(summary.target) << " bp\n";
+    if (summary.status == 1) std::cerr << "  not enough reads to reach target\n";
+    else if (summary.status == 2) std::cerr << "  reads already fall below target after filtering\n";
+    else std::cerr << "  keeping " << int_to_string(summary.keeping) << " bp\n";
+    std::cerr << "\n";
+}

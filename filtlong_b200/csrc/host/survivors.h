@@ -1,0 +1,82 @@
+// filtlong_b200/csrc/host/survivors.h -- pass 2 of the CLI: the surviving reads and child rows in input order, as the
+// reference prints them (reference src/main.cpp:263-313), and the stderr blocks that lead up to it. The only code that
+// knows that output layout and how the bytes reach the descriptor. Two sources feed it:
+//   * random access: the mapped input and a table of where each record sits (the device feeder's, one part per shard, or
+//     the host reader's when every record was simple). To BGZF; to pwrite() groups written by a few threads when the
+//     descriptor is a regular file not opened with O_APPEND; else to writev().
+//   * sequential: the input parsed again by FastxReader (streamed gzip, CR LF, multi-line records), copied through a
+//     buffer or into BGZF.
+// Every writer returns false when a write (or a compression) failed.
+#pragma once
+#include <cstdint>
+#include <string>
+#include <vector>
+
+#include "../../../include/filtlong_b200.h"
+#include "arguments.h"
+
+// Where each record sits in the mapped input, as file offsets. A comment starts one byte after its name (the device and
+// FastxReader both guarantee it).
+struct Records {
+    std::vector<uint64_t> name_off, seq_off, qual_off, name_hash;
+    std::vector<uint32_t> name_len, comment_len;
+    std::vector<int32_t> len;
+    size_t n = 0;
+    bool lead_checked = false;    // every name follows the format's lead character (the device checked it)
+    void ensure(size_t cap) {
+        if (name_off.size() >= cap) return;
+        const size_t c = cap + cap / 2;
+        name_off.resize(c); seq_off.resize(c); qual_off.resize(c); name_hash.resize(c);
+        name_len.resize(c); comment_len.resize(c); len.resize(c);
+    }
+    void add(uint64_t name_o, uint32_t name_l, uint32_t comment_l, uint64_t seq_o, uint64_t qual_o, int32_t length) {
+        ensure(n + 1);
+        name_off[n] = name_o; name_len[n] = name_l; comment_len[n] = comment_l;
+        seq_off[n] = seq_o; qual_off[n] = qual_o; len[n] = length;
+        ++n;
+    }
+    bool within(uint64_t file_size, bool quality) const;   // every piece that is printed lies inside the file
+};
+
+// Read-only view of the results pass 2 needs. ReadSet and the feeder's shards hold these arrays under these names.
+struct Results {
+    const int32_t *n_child;
+    const uint64_t *row_start;
+    const int32_t *row_s, *row_e;
+    const uint8_t *row_pfinal;
+    template <class T> static Results of(const T &t) {
+        return Results{t.n_child.data(), t.row_start.data(), t.row_s.data(), t.row_e.data(), t.row_pfinal.data()};
+    }
+};
+
+struct Format {
+    char lead;                    // '>' or '@'
+    bool quality;                 // print "+" and the quality
+};
+
+struct Part {                     // one part of the table, with its results
+    const Records *rec;
+    Results res;
+};
+
+// name_<start+1>-<end>, a child read's name (reference src/read.cpp:135-136), appended to `out`
+inline void append_child_name(std::string &out, const char *name, size_t name_len, int start, int end) {
+    out.append(name, name_len);
+    out += '_';
+    out += std::to_string(start + 1);
+    out += '-';
+    out += std::to_string(end);
+}
+
+// Random access: the survivors of `parts`, in order, from the input mapped at `base`; compressed on the context `bgzf`
+// when it is given. The last two are the choices write_survivors makes, callable directly.
+bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf);
+bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);
+bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);
+// Sequential: the survivors among the first n_reads records of `path`, parsed again.
+bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf);
+
+// "  after trimming / splitting: N reads (B bp)" when --trim or --split is on, then a blank line (main.cpp:157-167)
+void log_after_trim_split(const Arguments &args, uint64_t n_rows, const fl_summary &summary);
+// the "Filtering long reads" block, when a target is set (main.cpp:218-261)
+void log_filtering(const Arguments &args, const fl_summary &summary);

@@ -10,9 +10,9 @@ int main(int argc, char **argv) {
     if (!in.ok()) return 3;
     long long l;
     while ((l = in.next()) >= 0)
-        printf("%s\t%zu\t%zu\t%zu\t%d\t%llu\t%llu\t%llu\t%d\n", in.name.c_str(), in.comment.size(), in.seq.size(), in.qual.size(),
+        printf("%s\t%zu\t%zu\t%zu\t%d\t%llu\t%llu\t%llu\t%d\t%llu\n", in.name.c_str(), in.comment.size(), in.seq.size(), in.qual.size(),
                (int)in.simple, (unsigned long long)in.comment_off, (unsigned long long)in.seq_off, (unsigned long long)in.qual_off,
-               (int)in.plain());
+               (int)in.plain(), (unsigned long long)in.name_off);
     printf("END %lld\n", l);
     return 0;
 }

@@ -118,3 +118,8 @@ def test_edge_cases(inputs, tmp_path):
     assert rc == 1
     rc, _, _ = run(["-p", "80", "--bgzip", inputs["CRLF"]], stdout_path="/dev/full")
     assert rc == 1
+    # plain output from the host reader: the re-parse (CR LF) and the mapped slices fail like the feeder's
+    rc, _, _ = run(["-p", "80", inputs["CRLF"]], stdout_path="/dev/full")
+    assert rc == 1
+    rc, _, _ = run(["-p", "80", inputs["FQ"]], env_extra={"FL_HOST_PARSER": "1"}, stdout_path="/dev/full")
+    assert rc == 1

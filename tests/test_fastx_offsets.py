@@ -1,6 +1,6 @@
 """FastxReader's stream offsets (used by the CLI's pass 2 to copy slices of the input instead of parsing
 it again, main.cpp:263-313): for every record it calls `simple`, the file's bytes at the reported
-offsets are exactly the comment, the sequence and the quality it parsed; records it cannot vouch for
+offsets are exactly the name, the comment, the sequence and the quality it parsed; records it cannot vouch for
 (multi-line, CR LF) are flagged; gzip input is reported as not plain."""
 import gzip
 import os
@@ -69,7 +69,10 @@ def test_offsets_point_at_the_parsed_pieces(dumper, style, tmp_path):
         assert f[8] == "1"
         if f[4] == "1":
             n_simple += 1
-            co, so, qo = int(f[5]), int(f[6]), int(f[7])
+            no, co, so, qo = int(f[9]), int(f[5]), int(f[6]), int(f[7])
+            assert data[no - 1:no + len(name)] == b"@" + name
+            if comment:                                   # pass 2 looks for the comment one byte after the name
+                assert co == no + len(name) + 1
             assert data[co:co + len(comment)] == comment
             assert data[so:so + len(seq)] == seq
             assert data[qo:qo + len(qual)] == qual
@@ -90,8 +93,9 @@ def test_fasta_and_gzip(dumper, tmp_path):
     lines = subprocess.run([dumper, path], capture_output=True, text=True).stdout.splitlines()
     f1, f2, f3 = (l.split("\t") for l in lines[:3])
     assert f1[4] == "1" and data[int(f1[6]):int(f1[6]) + 8] == b"ACGTACGT" and data[int(f1[5]):int(f1[5]) + 12] == b"first contig"
+    assert data[int(f1[9]):int(f1[9]) + 2] == b"c1" and int(f1[5]) == int(f1[9]) + 3
     assert f2[4] == "0" and int(f2[2]) == 4
-    assert f3[4] == "1" and data[int(f3[6]):int(f3[6]) + 4] == b"TTTT"
+    assert f3[4] == "1" and data[int(f3[6]):int(f3[6]) + 4] == b"TTTT" and data[int(f3[9]) - 1:int(f3[9]) + 2] == b">c3"
     gz = str(tmp_path / "r.fastq.gz")
     with gzip.open(gz, "wb") as f:
         f.write(b"@r1\nACGT\n+\nIIII\n")
