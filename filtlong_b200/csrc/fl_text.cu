@@ -31,19 +31,41 @@ __device__ __forceinline__ uint32_t nl_mask16(const uint4 v, int nvalid) {
     return m;
 }
 
-// pass A: newlines per 512-byte block
+// does any of the first nvalid bytes of the 16 hold a NUL?
+__device__ __forceinline__ bool has_nul16(const uint4 v, int nvalid) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t m = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const uint32_t eq = __vcmpeq4(w[i], 0u) & 0x01010101u;
+        m |= ((eq | (eq >> 7) | (eq >> 14) | (eq >> 21)) & 0xFu) << (4 * i);
+    }
+    if (nvalid < 16) m &= (1u << (nvalid < 0 ? 0 : nvalid)) - 1u;
+    return m != 0;
+}
+
+// pass A: newlines per 512-byte block; *nul set when the text holds a NUL byte. The reference handles every field as a
+// C string (main.cpp:90,268-305: a name, comment, sequence or quality ends at its first NUL for the dictionary and the
+// output), which slices of the text cannot reproduce: such a chunk is the host reader's.
 __global__ void __launch_bounds__(256) k_text_count(const uint8_t *__restrict__ text, unsigned long long n_bytes, unsigned long long n_blocks,
-                                                    unsigned long long *__restrict__ counts) {
+                                                    unsigned long long *__restrict__ counts, int *__restrict__ nul) {
     const unsigned lane = threadIdx.x & 31;
     const unsigned long long warp = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5,
                              n_warps = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
+    bool z = false;
     for (unsigned long long b = warp; b < n_blocks; b += n_warps) {
         const unsigned long long pos = b * TX_LINES_PER_WARP + 16ull * lane;
         uint32_t m = 0;
-        if (pos < n_bytes) m = nl_mask16(__ldg(reinterpret_cast<const uint4 *>(text + pos)), (int)(n_bytes - pos < 16 ? n_bytes - pos : 16));
+        if (pos < n_bytes) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(text + pos));
+            const int nvalid = (int)(n_bytes - pos < 16 ? n_bytes - pos : 16);
+            m = nl_mask16(v, nvalid);
+            z |= has_nul16(v, nvalid);
+        }
         const int c = __reduce_add_sync(0xffffffffu, __popc(m));
         if (lane == 0) counts[b] = (unsigned long long)c;
     }
+    if (z) atomicOr(nul, 1);
 }
 
 // pass B: positions of the newlines, in order (counts[] now holds the exclusive scan)
@@ -109,6 +131,7 @@ __global__ void __launch_bounds__(256) k_text_records(RecArgs a) {
     if (nlen == 0) bad = true;
     const unsigned long long clen = p < e0 ? e0 - (p + 1) : 0ull;
     if (e1 <= s1) bad = true;                                            // empty sequence line
+    else if (a.text[s1] == '@' || a.text[s1] == '>' || a.text[s1] == '+') bad = true;   // kseq.h:199: ends the sequence there
     const unsigned long long L = e1 > s1 ? e1 - s1 : 0ull;
     if (L > 0x7FFFFFFFull) bad = true;                                   // main.cpp:69,77: int length
     unsigned long long s3 = 0;
@@ -245,6 +268,7 @@ __global__ void __launch_bounds__(256) k_fa_heads(FaArgs a) {
     else {
         if (a.text[e - 1] == '\r') bad = true;                      // CR LF
         if (!h && (a.text[s] == '@' || a.text[s] == '+')) bad = true;   // kseq.h:199: ends the sequence
+        if (h && e - s == 1 && i >= a.n_lines) bad = true;          // a '>' that ends the file starts no record (kseq.h:193, -1)
     }
     if (bad) atomicOr(a.bad, 1);
 }
@@ -357,6 +381,7 @@ struct TextLines {
     unsigned long long n_blocks = 0, n_lines = 0, n_lines_virtual = 0;
     unsigned grid = 0;
     bool ends_with_nl = false;
+    bool has_nul = false;             // a NUL byte anywhere in the chunk: not the layout
 };
 
 static int text_lines(fl_ctx *c, const char *host_text, uint64_t n_bytes, int is_last_chunk, TextLines &tl) {
@@ -379,12 +404,16 @@ static int text_lines(fl_ctx *c, const char *host_text, uint64_t n_bytes, int is
     FL_CUDA(c, c->sc_u64a.reserve(tl.n_blocks + 1, 0, st));
     tl.grid = fl_blocks(tl.n_blocks * 32, 256);
     if (tl.grid > (unsigned)c->sm_count * 16) tl.grid = (unsigned)c->sm_count * 16;
-    k_text_count<<<tl.grid, 256, 0, st>>>(text, n_bytes, tl.n_blocks, c->sc_u64a.p);
+    int *d_nul = reinterpret_cast<int *>(c->d_scalars + 29);
+    FL_CUDA(c, cudaMemsetAsync(d_nul, 0, sizeof(unsigned long long), st));
+    k_text_count<<<tl.grid, 256, 0, st>>>(text, n_bytes, tl.n_blocks, c->sc_u64a.p, d_nul);
     c->launches++;
     FL_TRY(fl_exclusive_scan_u64(c, c->sc_u64a.p, c->sc_u64a.p, tl.n_blocks, c->d_scalars));
     FL_CUDA(c, cudaMemcpyAsync(c->h_scalars, c->d_scalars, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     FL_CUDA(c, cudaMemcpyAsync(c->h_scalars + 1, text + n_bytes - 1, 1, cudaMemcpyDeviceToHost, st));
+    FL_CUDA(c, cudaMemcpyAsync(c->h_scalars + 6, d_nul, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     FL_CUDA(c, cudaStreamSynchronize(st));
+    tl.has_nul = c->h_scalars[6] != 0;
     tl.n_lines = c->h_scalars[0];
     tl.ends_with_nl = (reinterpret_cast<const unsigned char *>(c->h_scalars + 1))[0] == '\n';
     tl.n_lines_virtual = tl.n_lines + ((is_last_chunk && !tl.ends_with_nl) ? 1 : 0);   // the file's last line may lack its newline
@@ -409,9 +438,10 @@ static int text_index(fl_ctx *c, const char *host_text, uint64_t n_bytes, int lp
     const uint8_t *text = tl.text;
     ix.text = text;
     const unsigned long long n_lines = tl.n_lines, n_lines_virtual = tl.n_lines_virtual;
-    if (lpr == 2 && (n_lines_virtual & 1ull)) {
-        // FASTA: a line left over after the last pair may continue that record's sequence (a wrapped record): the
-        // record is not what it seems, and kseq would read on. Not the simple layout.
+    if (tl.has_nul || (lpr == 2 && (n_lines_virtual & 1ull))) {
+        // a NUL (see k_text_count), or FASTA with
+        // a line left over after the last pair, which may continue that record's sequence (a wrapped
+        // record): the record is not what it seems, and kseq would read on. Not the simple layout.
         FL_CUDA(c, cudaStreamSynchronize(c->copy_stream));
         *status = FL_TEXT_FALLBACK;
         ix.done = true;
@@ -484,7 +514,7 @@ static int fasta_index(fl_ctx *c, const char *host_text, uint64_t n_bytes, int i
     };
     const unsigned long long NL = tl.n_lines_virtual;
     // a chunk that is not the file's last must end with a newline (the caller cuts at record starts), and there must be lines
-    if (NL == 0 || NL > 0xFFFFFFF0ull || (!tl.ends_with_nl && !is_last_chunk)) return fallback();
+    if (tl.has_nul || NL == 0 || NL > 0xFFFFFFF0ull || (!tl.ends_with_nl && !is_last_chunk)) return fallback();
     FL_TRY(text_positions(c, n_bytes, tl));
     FL_CUDA(c, c->sc_u64c.reserve((size_t)NL + 1, 0, st));
     FaArgs a{};

@@ -22,6 +22,10 @@ FastxReader::~FastxReader() {
     delete[] buf_;
 }
 
+// pass 2 prints the comment, the sequence and the quality as C strings (main.cpp:273-305): a record with a NUL is
+// not a slice of the input
+static bool has_nul(const std::string &s) { return !s.empty() && memchr(s.data(), 0, s.size()) != nullptr; }
+
 int FastxReader::getc() {
     if (err_) return -3;
     if (eof_ && begin_ >= end_) return -1;
@@ -84,6 +88,12 @@ int64_t FastxReader::next() {
     }
     if (!got) return c == -3 ? -3 : -1;
     simple = true;
+    // the reference uses the name only as a C string (main.cpp:81,90,99,114,268,273): it ends at the first NUL
+    const size_t nul = name.find('\0');
+    if (nul != std::string::npos) {
+        name.resize(nul);
+        simple = false;
+    }
     comment_off = pos();
     if (c >= 0 && c != '\n') {
         get_line(comment, false);
@@ -102,6 +112,7 @@ int64_t FastxReader::next() {
     is_fastq = (c == '+');
     if (!is_fastq) {
         if (c != '>' && c != '@') last_char_ = 0;   // end of file
+        if (has_nul(comment) || has_nul(seq)) simple = false;
         return (int64_t)seq.size();
     }
     while ((c = getc()) >= 0 && c != '\n') {}
@@ -119,5 +130,6 @@ int64_t FastxReader::next() {
     if (err_) return -2;
     last_char_ = 0;
     if (seq.size() != qual.size()) return -2;
+    if (has_nul(comment) || has_nul(seq) || has_nul(qual)) simple = false;
     return (int64_t)seq.size();
 }

@@ -11,6 +11,9 @@
 //     are at least as long as the sequence;
 //   - next() returns the sequence length, or -1 at end of file, -2 for a truncated / mismatching
 //     quality string, -3 on a stream error.
+// One rule comes from the reference's use of kseq rather than kseq itself: `name` ends at its first NUL
+// byte, because the reference only ever reads it as a C string. The comment, the sequence and the quality
+// keep every byte (the reference scores seq.l bases); pass 2 prints them up to their first NUL.
 #pragma once
 #include <zlib.h>
 
@@ -33,7 +36,8 @@ public:
     // slices of the input instead of parsing it a second time (main.cpp:263-313 re-reads the file).
     // Valid after next() >= 0. `simple` says the sequence and the quality each came from exactly one
     // line with nothing stripped, i.e. input[seq_off, seq_off + length) IS the sequence (and likewise
-    // for the name, the quality and the comment); otherwise the offsets must not be used.
+    // for the name, the quality and the comment, none of which holds a NUL); otherwise the offsets
+    // must not be used.
     bool simple = false;
     uint64_t name_off = 0, comment_off = 0, seq_off = 0, qual_off = 0;
     // true when the file is not compressed: stream offsets are file offsets

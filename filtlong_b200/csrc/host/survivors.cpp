@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cstdio>
+#include <cstring>
 #include <iostream>
 #include <thread>
 
@@ -36,13 +37,22 @@ struct RecordText {               // one input record's bytes
     const char *seq, *qual;
     size_t len;
     bool lead_before_name;        // name[-1] is the format's lead character
+    // The reference prints the comment when it has any byte, but prints it, the sequence and the quality as C strings
+    // (main.cpp:274-305). These are the printed lengths: up to the first NUL (all of it when there is none).
+    bool has_comment;
+    size_t comment_print, seq_print, qual_print;
 };
 
 RecordText text_of(const Records &R, const char *base, size_t i) {
     const char *name = base + R.name_off[i];
-    return RecordText{name, R.name_len[i], name + R.name_len[i] + 1, R.comment_len[i], base + R.seq_off[i], base + R.qual_off[i],
-                      (size_t)R.len[i], R.lead_checked};
+    const size_t L = (size_t)R.len[i], C = R.comment_len[i];
+    return RecordText{name, R.name_len[i], name + R.name_len[i] + 1, C, base + R.seq_off[i], base + R.qual_off[i], L, R.lead_checked,
+                      C > 0, C, L, L};
 }
+
+// bytes [start, start + length) of a C string of n bytes, as std::string(s).substr(start, length) gives them. Past its
+// end the reference's substr throws; here nothing is printed (DESIGN 5).
+size_t c_substr(size_t n, size_t start, size_t length) { return start >= n ? 0 : std::min(length, n - start); }
 
 // Read i's output: the read if it survived and has no children, else each surviving child longer than 0. put()'s bytes
 // must stay valid until the sink is flushed; put_owned() keeps its string alive until then.
@@ -50,11 +60,11 @@ template <class Sink>
 void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Results &res, size_t i) {
     const char *lead = fmt.lead == '>' ? ">" : "@";
     auto rest = [&](size_t start, size_t length) {
-        if (r.comment_len) { sink.put(" ", 1); sink.put(r.comment, r.comment_len); }
+        if (r.has_comment) { sink.put(" ", 1); sink.put(r.comment, r.comment_print); }
         sink.put("\n", 1);
-        sink.put(r.seq + start, length);
+        sink.put(r.seq + start, c_substr(r.seq_print, start, length));
         sink.put("\n", 1);
-        if (fmt.quality) { sink.put("+\n", 2); sink.put(r.qual + start, length); sink.put("\n", 1); }
+        if (fmt.quality) { sink.put("+\n", 2); sink.put(r.qual + start, c_substr(r.qual_print, start, length)); sink.put("\n", 1); }
     };
     const size_t rs = (size_t)res.row_start[i];
     if (res.n_child[i] == 0) {
@@ -219,7 +229,8 @@ bool reparse_survivors(int fd, const std::string &path, const Results &res, size
     auto run = [&](auto &sink) {
         for (size_t i = 0; in.ok() && in.next() >= 0 && i < n_reads; ++i) {
             const RecordText r{in.name.data(), in.name.size(), in.comment.data(), in.comment.size(), in.seq.data(), in.qual.data(),
-                               in.seq.size(), false};
+                               in.seq.size(), false, !in.comment.empty(), strnlen(in.comment.data(), in.comment.size()),
+                               strnlen(in.seq.data(), in.seq.size()), strnlen(in.qual.data(), in.qual.size())};
             emit_survivors(sink, fmt, r, res, i);
         }
     };

@@ -62,13 +62,16 @@ inline uint64_t eol(const char *b, uint64_t from, uint64_t size) {
     return p ? (uint64_t)((const char *)p - b) : size;
 }
 
-// Is `p` the first byte of a record? FASTQ: '@' line, a sequence line, a '+' line, a quality line as long as the
-// sequence (a quality line that begins with '@' fails the '+' test two lines on). FASTA: any line starting with '>'.
+// Is `p` the first byte of a record? FASTQ: '@' line, a sequence line that kseq takes for one (not empty, not led by
+// '@', '>' or '+': kseq.h:199), a '+' line, a quality line as long as the sequence (a quality line that begins with '@'
+// fails the '+' test two lines on). FASTA: any line starting with '>'. A cut the device then rejects costs only the
+// fast path: the host reader takes over at the chunk's first byte.
 bool record_starts_at(const char *b, uint64_t p, uint64_t size, int format) {
     if (p >= size) return false;
     if (format == FL_TEXT_FASTA) return b[p] == '>';
     if (b[p] != '@') return false;
     const uint64_t e0 = eol(b, p, size), s1 = e0 + 1, e1 = eol(b, s1, size), s2 = e1 + 1;
+    if (e1 <= s1 || b[s1] == '@' || b[s1] == '>' || b[s1] == '+') return false;
     if (s2 >= size || b[s2] != '+') return false;
     const uint64_t e2 = eol(b, s2, size), s3 = e2 + 1, e3 = eol(b, s3, size);
     return s3 <= size && e3 - s3 == e1 - s1;
