@@ -107,7 +107,7 @@ struct SelectState {
     long long passed_bases;          // global
     long long total_bases;           // global
     int status;                      // fl_summary.status
-    int active;                      // 1 while digits are still being resolved
+    int active;                      // 1 while digits are still being resolved (status 3 and target > 0)
     unsigned long long tie_key;      // full key of the tie class at the cut-off
     unsigned long long tie_base;     // bases the tie class may still take: target - cum_before
 };

@@ -39,8 +39,11 @@ def main():
     rows = ctx.row_results()
     np.savez(os.path.join(wd, "out_%d.npz" % rank), lo=lo, hi=hi, n_kmers=n_k, passed_final=rows["passed_final"], start=rows["start"],
              end=rows["end"], final_score=rows["final_score"], mean_q=rows["mean_q"], window_q=rows["window_q"],
-             summary=np.array([summ.status, summ.target, summ.keeping, summ.passed_bases, summ.total_bases], dtype=np.int64),
-             stats=np.array([summ.min_q, summ.max_q, summ.mean_q, summ.stdev_q]), collectives=ctx.collective_count())
+             passed=rows["passed"], length_score=rows["length_score"], norm_mean=rows["norm_mean"], norm_window=rows["norm_window"],
+             summary=np.array([summ.status, summ.target, summ.keeping, summ.passed_bases, summ.total_bases, summ.rows_bases],
+                              dtype=np.int64),
+             stats=np.array([summ.min_q, summ.max_q, summ.mean_q, summ.stdev_q, summ.min_z, summ.max_z]),
+             collectives=ctx.collective_count())
     ctx.comm_destroy()
     ctx.close()
 

@@ -18,6 +18,17 @@ def score_keys(final):
     return k
 
 
+def target_and_status(p, total, passed_bases):
+    """main.cpp:229-244: the signed target and the status (0 no target, 1 not enough reads, 2 already
+    below the target, 3 cut). The target is 0 when neither option is set, as fl_summary reports it."""
+    if not (p.target_bases_set or p.keep_percent_set):
+        return 0, 0
+    target = p.target_bases if p.target_bases_set else (1 << 63) - 1
+    if p.keep_percent_set:
+        target = min(target, int((p.keep_percent / 100.0) * total))
+    return target, (1 if target >= total else (2 if target >= passed_bases else 3))
+
+
 class NumpyPhases:
     def __init__(self, mean, window, length, passed, params):
         self.mean = np.asarray(mean, dtype=np.float64)
@@ -69,13 +80,9 @@ class NumpyPhases:
     def select_begin(self, total, sums):
         st = self.state
         p = self.p
-        st.any = bool(p.target_bases_set or p.keep_percent_set)
-        target = p.target_bases if p.target_bases_set else (1 << 63) - 1
-        if p.keep_percent_set:
-            target = min(target, int((p.keep_percent / 100.0) * total))
-        st.target, st.total, st.passed_bases = target, total, int(sums.numpy()[2])
-        st.status = 0 if not st.any else (1 if target >= total else (2 if target >= st.passed_bases else 3))
-        st.active = st.status == 3
+        st.passed_bases, st.total = int(sums.numpy()[2]), total
+        st.target, st.status = target_and_status(p, total, st.passed_bases)
+        st.active = st.status == 3 and st.target > 0          # a target <= 0 keeps nothing
         st.prefix, st.cum = 0, 0
 
     def select_hist(self, level, hist):
@@ -115,6 +122,8 @@ class NumpyPhases:
     def select_apply(self, tie, rank, keeping):
         st = self.state
         keeping.numpy()[0] = 0
+        if st.status == 3 and not st.active:
+            self.pfinal = np.zeros_like(self.passed)
         if not st.active:
             return
         before = int(tie.numpy()[:rank].sum())
@@ -130,5 +139,5 @@ class NumpyPhases:
 
     def select_summary(self, sums, mn, mx, sq, keeping, total):
         st = self.state
-        return types.SimpleNamespace(status=st.status, target=st.target if st.any else 0, passed_bases=st.passed_bases,
+        return types.SimpleNamespace(status=st.status, target=st.target, passed_bases=st.passed_bases,
                                      keeping=int(keeping.numpy()[0]) if st.status == 3 else 0, total_bases=total)

@@ -4,6 +4,8 @@ import struct
 
 import numpy as np
 
+from tests import select_model as sm
+
 SCORE_RTOL = 1e-5      # north star: combined float scores within 1e-5 relative
 TIE_RTOL = 1e-9        # rows this close at the cut-off are a tie class (SURVEY H1/H2)
 
@@ -87,3 +89,49 @@ def check_selection(got, want, ref_scores, lengths):
     if not math.isnan(lo):
         assert hi - lo <= TIE_RTOL * max(abs(hi), 1e-300), "selection differs outside a tie class: %r" % (diff[:10],)
     assert sum(l for l, g in zip(lengths, got) if g) == sum(l for l, w in zip(lengths, want) if w)
+
+
+# ---------------------------------------------------------------------------------------------
+# exact checks of the last stage against the device's own statistics (tests/select_model.py)
+# ---------------------------------------------------------------------------------------------
+def _same_bits(a, b):
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    return (a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))
+
+
+def row_lengths(rw):
+    return (np.asarray(rw["end"], np.int64) - np.asarray(rw["start"], np.int64))
+
+
+def check_rescale_exact(rw, summary, params, nranks=1):
+    """rw: Context.row_results() (all ranks' rows, in order); summary: the fl_summary of that finalize.
+    length_score, norm_mean and norm_window bit-identical to the restatement fed with the summary's
+    statistics; final_score too where every pow() is exact, else within select_model.final_ulp_bound;
+    min_q / max_q bit-exact, mean_q / stdev_q within the summation tree's bound of the exact values;
+    passed and row bases exact."""
+    length = row_lengths(rw)
+    lw, mw, ww = params.length_weight, params.mean_q_weight, params.window_q_weight
+    want = sm.rescale(rw["mean_q"], rw["window_q"], length, summary, lw, mw, ww)
+    for k in ("length_score", "norm_mean", "norm_window"):
+        ok = _same_bits(rw[k], want[k])
+        bad = np.nonzero(~ok)[0]
+        assert bad.size == 0, (k, bad[:10], rw[k][bad[:5]], want[k][bad[:5]])
+    sm.check_final(rw["final_score"], want, lw, mw)
+    sm.check_stats(summary, rw["mean_q"], nranks)
+    passed = np.asarray(rw["passed"]).astype(bool)
+    assert summary.passed_bases == int(length[passed].sum())
+    assert summary.rows_bases == int(length.sum())
+
+
+def check_selection_exact(rw, summary, params):
+    """The device's pass flags, kept bases, target and status must be exactly the stable sort + signed
+    prefix walk over its own final scores (NaN first, equal keys in row order: the library's rule)."""
+    length = row_lengths(rw)
+    passed = np.asarray(rw["passed"]).astype(bool)
+    target, status = sm.target_and_status(params, summary.total_bases, int(length[passed].sum()))
+    assert (summary.target, summary.status) == (target, status), ((summary.target, summary.status), (target, status))
+    want, keeping = sm.expected_cut(rw["final_score"], passed, length, target, status)
+    got = np.asarray(rw["passed_final"], np.uint8)
+    bad = np.nonzero(got != want)[0]
+    assert bad.size == 0, ("passed_final", bad.size, bad[:10])
+    assert summary.keeping == keeping, (summary.keeping, keeping)

@@ -91,4 +91,6 @@ def test_cuda_path_reproduces_golden(path):
     parity.check_selection([int(x) for x in rw["passed_final"]], [gr["passed_final"] for gr in g["rows"]],
                            [float.fromhex(gr["final_score"]) for gr in g["rows"]], [gr["length"] for gr in g["rows"]])
     assert summ.keeping == g["tail"]["keeping"] and summ.status == g["tail"]["status"]
+    parity.check_rescale_exact(rw, summ, p)
+    parity.check_selection_exact(rw, summ, p)
     ctx.close()

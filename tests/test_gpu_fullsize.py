@@ -9,7 +9,9 @@
   must match the oracle bit-for-bit;
 * the selection must satisfy the reference's prefix-walk invariants (main.cpp:251-257): every kept
   row scores at least as high as every passed row that was dropped, kept bases reach the target and
-  would not reach it without the lowest-scoring kept row.
+  would not reach it without the lowest-scoring kept row;
+* the rescaling and the selection must be exactly the restatement of tests/select_model.py, fed with
+  the device's own statistics and scores (parity.check_rescale_exact / check_selection_exact).
 """
 import ctypes as C
 import os
@@ -106,6 +108,8 @@ def test_config2_phred_full_size():
         assert np.array_equal(rows["passed_final"], rows2["passed_final"]), other
         assert (s2.status, s2.target, s2.keeping) == (summ.status, summ.target, summ.keeping)
     _selection_invariants(rows, summ, target)
+    parity.check_rescale_exact(rows, summ, params)
+    parity.check_selection_exact(rows, summ, params)
     # the first reads AND the 50 longest ones (the 1 Mbase reads, where the lattice sum crosses the most
     # binades) against the oracle, regenerated on the host one read at a time (the generator is keyed by
     # the read's global index)
@@ -250,6 +254,8 @@ def test_config3_kmer_full_size():
     assert np.all(rows["start"][1:][same_parent] >= rows["end"][:-1][same_parent])
     assert int((rows["end"] - rows["start"]).astype(np.int64).sum()) == summ.rows_bases
     _selection_invariants(rows, summ, summ.target)
+    parity.check_rescale_exact(rows, summ, params)
+    parity.check_selection_exact(rows, summ, params)
     # the first reads and the 50 longest against the oracle (host-regenerated reads; the oracle's Kmers is
     # loaded with the exported set: the CPU cannot hash 10 M short reads inside a test)
     idx = np.concatenate([np.arange(400), np.argsort(-w["len"].astype(np.int64), kind="stable")[:50]])
@@ -323,8 +329,8 @@ def test_sharded_kmer_run_equals_single_context_run():
         c.push_device(api.device_batch(hi - lo, end - base, rel, t_len[lo:hi], seq2b=d_seq[base // 16:]))
     # the split-phase protocol with the all-reduces done by hand on the device buffers: the transport-agnostic
     # form of what fl_finalize does over NCCL (that path is exercised on >= 2 GPUs by test_nccl_two_ranks)
-    from tests.test_gpu_parity import _two_shard_finalize
-    summaries = _two_shard_finalize(ctxs, w["bases"])
+    from tests import util
+    summaries = util.split_phase_finalize(ctxs, w["bases"])
     rows2 = [c.row_results() for c in ctxs]
     cat = {k: np.concatenate([r[k] for r in rows2]) for k in ("start", "end", "passed_final", "mean_q", "window_q", "final_score")}
     for k in ("start", "end", "passed_final"):

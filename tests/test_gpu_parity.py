@@ -1,7 +1,8 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the oracle on the same seeded
 inputs. Per-read values (raw mean / window quality, first/last base, bad and child ranges, hard
 pass flags) must be bit-identical; normalised / final scores within 1e-5 relative (north star);
-selected row IDs identical (modulo the tie class at the cut-off, tests/parity.py)."""
+selected row IDs identical (modulo the tie class at the cut-off, tests/parity.py). Judged by the
+device's own statistics instead, the rescaling and the cut are exact (tests/select_model.py)."""
 import numpy as np
 import pytest
 
@@ -30,6 +31,9 @@ def full_check(ctx, summ, sc):
     rr, rw = ctx.read_results(), ctx.row_results()
     parity.check_reads_vs_oracle(rr, sc)
     parity.check_rows_vs_oracle(rw, rr, sc, summ)
+    # and exactly, against the device's own statistics and scores
+    parity.check_rescale_exact(rw, summ, ctx.params)
+    parity.check_selection_exact(rw, summ, ctx.params)
 
 
 PHRED_CASES = [
@@ -395,51 +399,6 @@ def test_kmer_results_do_not_depend_on_batching():
     assert outs[0] == outs[1] == outs[2]
 
 
-def _two_shard_finalize(ctxs, total_bases):
-    """Runs the split-phase normalise/select protocol of filtlong_b200/sharding.py over two contexts
-    on ONE GPU, with the all-reduces done by hand on the device buffers (what NCCL does between
-    ranks). Returns the per-context summaries."""
-    import torch
-    from filtlong_b200 import sharding
-    world = len(ctxs)
-    bks = [sharding.CabiBackend(c) for c in ctxs]
-    bufs = [sharding.Buffers(torch, "cuda", world) for _ in ctxs]
-
-    def allreduce(name, op="sum"):
-        ts = [getattr(b, name) for b in bufs]
-        for c in ctxs:
-            c.sync()
-        torch.cuda.synchronize()
-        st = torch.stack(ts)
-        red = st.sum(0) if op == "sum" else (st.min(0).values if op == "min" else st.max(0).values)
-        for t in ts:
-            t.copy_(red)
-        torch.cuda.synchronize()
-
-    for bk, b in zip(bks, bufs):
-        bk.norm_partial1(b.sums, b.mn, b.mx)
-    allreduce("sums"); allreduce("mn", "min"); allreduce("mx", "max")
-    for bk, b in zip(bks, bufs):
-        bk.norm_partial2(b.sums, b.mn, b.mx, b.sq)
-    allreduce("sq")
-    for bk, b in zip(bks, bufs):
-        bk.norm_apply(b.sums, b.mn, b.mx, b.sq)
-        bk.select_begin(total_bases, b.sums)
-    for level in range(8):
-        for bk, b in zip(bks, bufs):
-            bk.select_hist(level, b.hist)
-        allreduce("hist")
-        for bk, b in zip(bks, bufs):
-            bk.select_pick(level, b.hist)
-    for rank, (bk, b) in enumerate(zip(bks, bufs)):
-        bk.select_tie_local(b.tie, rank, world)
-    allreduce("tie")
-    for rank, (bk, b) in enumerate(zip(bks, bufs)):
-        bk.select_apply(b.tie, rank, b.keeping)
-    allreduce("keeping")
-    return [bk.select_summary(b.sums, b.mn, b.mx, b.sq, b.keeping, total_bases) for bk, b in zip(bks, bufs)]
-
-
 @pytest.mark.parametrize("opts,dup", [(dict(keep_percent=60.0), False), (dict(target_bases=250000, min_length=300), False),
                                       (dict(keep_percent=40.0), True)])
 def test_sharded_split_phase_protocol_on_device(opts, dup):
@@ -462,10 +421,14 @@ def test_sharded_split_phase_protocol_on_device(opts, dup):
         c = api.Context(p)
         c.push(api.HostBatch([r[0] for r in reads[lo:hi]], [r[1] for r in reads[lo:hi]], want_seq=False))
         ctxs.append(c)
-    summaries = _two_shard_finalize(ctxs, total)
+    summaries = util.split_phase_finalize(ctxs, total)
     got = []
-    for c in ctxs:
-        got += [int(x) for x in c.row_results()["passed_final"]]
+    rows = [c.row_results() for c in ctxs]
+    for r in rows:
+        got += [int(x) for x in r["passed_final"]]
+    cat = {k: np.concatenate([r[k] for r in rows]) for k in rows[0]}
+    parity.check_rescale_exact(cat, summaries[0], p, nranks=2)
+    parity.check_selection_exact(cat, summaries[0], p)
     parity.check_selection(got, [r.passed_final for r in sc.rows], [r.final_score for r in sc.rows], [r.length for r in sc.rows])
     for s in summaries:
         assert s.status == sc.summary.status

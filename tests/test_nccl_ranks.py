@@ -5,6 +5,7 @@ The union of the ranks' rows must equal what one context computes on the whole r
 import os
 import subprocess
 import sys
+import types
 
 import numpy as np
 import pytest
@@ -62,5 +63,14 @@ def test_nccl_ranks_equal_single_context(mode, opts, tmp_path):
         assert all(int(x["n_kmers"]) == len(ok) for x in z)
     sc = orc.finalize(orc.score([(s, q if not assembly else None) for s, q in reads], op, ok), op)
     got = [int(v) for v in np.concatenate([x["passed_final"] for x in z])]
+    # exact, against the ranks' own statistics and scores (every rank holds the same summary)
+    cat = {k: np.concatenate([x[k] for x in z]) for k in ("start", "end", "passed", "passed_final", "mean_q", "window_q",
+                                                          "length_score", "norm_mean", "norm_window", "final_score")}
+    sv, st = z[0]["summary"], z[0]["stats"]
+    s0 = types.SimpleNamespace(status=int(sv[0]), target=int(sv[1]), keeping=int(sv[2]), passed_bases=int(sv[3]),
+                               total_bases=int(sv[4]), rows_bases=int(sv[5]), min_q=st[0], max_q=st[1], mean_q=st[2],
+                               stdev_q=st[3], min_z=st[4], max_z=st[5])
+    parity.check_rescale_exact(cat, s0, p, nranks=n)
+    parity.check_selection_exact(cat, s0, p)
     parity.check_selection(got, [r.passed_final for r in sc.rows], [r.final_score for r in sc.rows], [r.length for r in sc.rows])
     one.close()

@@ -132,3 +132,48 @@ def read_fastx(path):
         else:
             i += 1
     return recs
+
+
+def split_phase_finalize(ctxs, total_bases):
+    """Runs the split-phase normalise/select protocol of filtlong_b200/sharding.py over N contexts (rank =
+    position in `ctxs`) on ONE GPU, with the all-reduces done by hand on the device buffers (what NCCL does
+    between ranks). Returns the per-context summaries."""
+    import torch
+    from filtlong_b200 import sharding
+    world = len(ctxs)
+    bks = [sharding.CabiBackend(c) for c in ctxs]
+    bufs = [sharding.Buffers(torch, "cuda", world) for _ in ctxs]
+
+    def allreduce(name, op="sum"):
+        ts = [getattr(b, name) for b in bufs]
+        for c in ctxs:
+            c.sync()
+        torch.cuda.synchronize()
+        st = torch.stack(ts)
+        red = st.sum(0) if op == "sum" else (st.min(0).values if op == "min" else st.max(0).values)
+        for t in ts:
+            t.copy_(red)
+        torch.cuda.synchronize()
+
+    for bk, b in zip(bks, bufs):
+        bk.norm_partial1(b.sums, b.mn, b.mx)
+    allreduce("sums"); allreduce("mn", "min"); allreduce("mx", "max")
+    for bk, b in zip(bks, bufs):
+        bk.norm_partial2(b.sums, b.mn, b.mx, b.sq)
+    allreduce("sq")
+    for bk, b in zip(bks, bufs):
+        bk.norm_apply(b.sums, b.mn, b.mx, b.sq)
+        bk.select_begin(total_bases, b.sums)
+    for level in range(8):
+        for bk, b in zip(bks, bufs):
+            bk.select_hist(level, b.hist)
+        allreduce("hist")
+        for bk, b in zip(bks, bufs):
+            bk.select_pick(level, b.hist)
+    for rank, (bk, b) in enumerate(zip(bks, bufs)):
+        bk.select_tie_local(b.tie, rank, world)
+    allreduce("tie")
+    for rank, (bk, b) in enumerate(zip(bks, bufs)):
+        bk.select_apply(b.tie, rank, b.keeping)
+    allreduce("keeping")
+    return [bk.select_summary(b.sums, b.mn, b.mx, b.sq, b.keeping, total_bases) for bk, b in zip(bks, bufs)]
