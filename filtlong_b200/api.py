@@ -108,6 +108,13 @@ class Context:
         self._ck(self.L.fl_ctx_kernel_time(self.h, self.KERNELS[name], C.byref(ms), C.byref(n)), "fl_ctx_kernel_time")
         return ms.value, n.value
 
+    def phred_paths(self):
+        """k_phred_win's path counters (fl_ctx_phred_paths): {path: (reads, bases)} and the exact steps walked."""
+        out = np.zeros(9, dtype=np.uint64)
+        self._ck(self.L.fl_ctx_phred_paths(self.h, out.ctypes.data), "fl_ctx_phred_paths")
+        paths = {k: (int(out[2 * i]), int(out[2 * i + 1])) for i, k in enumerate(("candidates", "full_walk", "reject_byte", "reject_low"))}
+        return paths, int(out[8])
+
     # ---- Kmers (kmers.h:28-55) ----
     def kmers_add(self, seqs, multiple_copies, chunk=200000):
         for i in range(0, len(seqs), chunk):

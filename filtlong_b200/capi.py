@@ -121,6 +121,7 @@ SYMBOLS = [
     ("fl_ctx_enable_timing", C.c_int, [_P, C.c_int]),
     ("fl_ctx_reset_timing", C.c_int, [_P]),
     ("fl_ctx_kernel_time", C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
+    ("fl_ctx_phred_paths", C.c_int, [_P, _P]),
     ("fl_padded_len", C.c_uint64, [C.c_int64]),
     ("fl_anchor_slot_host", None, [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     ("fl_pack_sequence", None, [C.c_char_p, C.c_char_p, C.c_int64, C.c_uint64, _P, _P, _P]),

@@ -162,6 +162,14 @@ extern "C" int fl_ctx_kernel_time(fl_ctx *c, int which, double *total_ms, uint64
     return FL_OK;
 }
 
+extern "C" int fl_ctx_phred_paths(fl_ctx *c, uint64_t out[9]) {
+    if (!c || !out) return FL_EINVAL;
+    FL_ENTER(c);
+    FL_CUDA(c, cudaStreamSynchronize(c->stream));
+    FL_CUDA(c, cudaMemcpy(out, c->d_scalars + FL_SCALAR_PHRED_PATHS, 9 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    return FL_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // host packer
 // ---------------------------------------------------------------------------------------------

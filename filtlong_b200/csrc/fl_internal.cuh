@@ -113,6 +113,7 @@ struct SelectState {
 };
 
 #define FL_HSCALAR_ROWS 40
+#define FL_SCALAR_PHRED_PATHS 30         // d_scalars[30, 39): k_phred_win's path counters (fl_ctx_phred_paths)
 
 struct fl_ctx {
     int device = 0;
@@ -188,7 +189,7 @@ struct fl_ctx {
     DevVec<uint32_t> sc_u32a;
     DevVec<unsigned long long> sc_scan;   // block sums of fl_exclusive_scan_u64
     uint32_t *d_buckets = nullptr;         // 256 bucket counters + 256 cursors (fl_order_by_length)
-    unsigned long long *d_scalars = nullptr;   // small device scalars (counts, cursors)
+    unsigned long long *d_scalars = nullptr;   // small device scalars (counts, cursors); [30, 39): FL_SCALAR_PHRED_PATHS
     unsigned long long *h_scalars = nullptr;   // pinned mirror
     // second half of a k-mer batch with --trim / --split, deferred by fl_reads_push (fl_score.cu: score_kmer_back)
     bool kmer_pending = false;

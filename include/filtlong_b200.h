@@ -108,6 +108,14 @@ enum { FL_KERNEL_SCORE_PHRED = 0, FL_KERNEL_PROBE_PAINT = 1, FL_KERNEL_KMER_STAT
 int fl_ctx_enable_timing(fl_ctx *ctx, int on);
 int fl_ctx_reset_timing(fl_ctx *ctx);
 int fl_ctx_kernel_time(fl_ctx *ctx, int which, double *total_ms, uint64_t *launches);
+/* Diagnostics: how the default Phred window kernel decided the minimum of the reads longer than the window,
+ * accumulated since the context was created. out[2p] counts reads and out[2p+1] their bases for path
+ * p = 0 (the candidate steps of the filter pass walked exactly), 1 (the whole chain walked exactly),
+ * 2 (sent to the sequential fallback by the filter pass: a quality byte the exact path cannot take, or a
+ * first window outside its range), 3 (sent there by the exact minimum: the window came near or below 0.5);
+ * out[8] is the number of exact steps walked.
+ * Synchronises the context's stream. */
+int fl_ctx_phred_paths(fl_ctx *ctx, uint64_t out[9]);
 
 /* Test hook (host): where the probe kernel looks for `kmer` when the 16-mer starts at a read position
  * whose low two bits are pos_lo2 -- 32-bit word index into the 2 GiB position-anchored table and the
