@@ -212,6 +212,16 @@ class Context:
         out.update(status="fallback" if st.value else "ok", n=n.value, consumed=used.value)
         return out
 
+    def push_bam(self, chunk: bytes, seq_off, qual_off, length):
+        """fl_reads_push_bam on a chunk of inflated BAM records: per record the chunk-relative offsets of SEQ and QUAL
+        and l_seq."""
+        so = np.ascontiguousarray(seq_off, dtype=np.uint32)
+        qo = np.ascontiguousarray(qual_off, dtype=np.uint32)
+        ln = np.ascontiguousarray(length, dtype=np.int32)
+        buf = np.frombuffer(chunk, dtype=np.uint8)
+        self._ck(self.L.fl_reads_push_bam(self.h, capi.ptr(buf), buf.size, ln.size, capi.ptr(so), capi.ptr(qo), capi.ptr(ln)),
+                 "fl_reads_push_bam")
+
     def kmers_add_text(self, data: bytes, fastq=True, is_last=True, multiple_copies=False):
         """fl_kmers_add_text on one chunk of a reference file (FASTQ / FASTA text)."""
         n, nb, used, st = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_int()

@@ -13,6 +13,7 @@
 // FL_TEXT_FALLBACK without scoring anything: the caller then runs its kseq-compatible host parser, which
 // reproduces the reference's behaviour (and error messages) on such input.
 #include "fl_device.cuh"
+#include "fl_name_hash.h"
 
 namespace {
 
@@ -121,12 +122,12 @@ __global__ void __launch_bounds__(256) k_text_records(RecArgs a) {
     if (e0 <= s0 || a.text[s0] != lead) bad = true;
     // name: up to the first whitespace; comment: the rest of the line after that one character (kseq.h:193-194)
     unsigned long long p = s0 + 1;
-    unsigned long long h = 0xCBF29CE484222325ull;                        // FNV-1a, then a final mix
+    unsigned long long h = FL_NAME_HASH_INIT;                            // fl_name_hash.h, shared with the BAM walker
     while (p < e0 && !tx_space(a.text[p])) {
-        h = (h ^ a.text[p]) * 0x100000001B3ull;
+        h = fl_name_hash_step(h, a.text[p]);
         ++p;
     }
-    h ^= h >> 29; h *= 0xBF58476D1CE4E5B9ull; h ^= h >> 32;
+    h = fl_name_hash_final(h);
     const unsigned long long nlen = p - (s0 + 1);
     if (nlen == 0) bad = true;
     const unsigned long long clen = p < e0 ? e0 - (p + 1) : 0ull;

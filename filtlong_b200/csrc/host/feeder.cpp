@@ -15,6 +15,7 @@
 #include <thread>
 #include <vector>
 
+#include "bam.h"
 #include "misc.h"
 #include "read.h"
 #include "survivors.h"
@@ -71,6 +72,7 @@ struct Ring {
     char *slot[KMAX] = {nullptr};
     bool registered[KMAX] = {false};
     int state[KMAX] = {0};                      // 0 free, 1 filled, -1 the reader failed
+    bool stop = false;                          // the shard stopped on its own (an error in the input): readers stop too
     std::mutex m;
     std::condition_variable cv;
 };
@@ -79,9 +81,81 @@ void check(fl_ctx *c, int rc, const char *what) {
     if (rc != FL_OK) throw std::runtime_error(std::string(what) + ": " + fl_last_error(c));
 }
 
+// A record of the input that fails a check. Only the shard that met it stops: the shards after it hold later records,
+// and the one before it may still meet an earlier one, whose message is the one printed.
+struct InputError : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+
+// How the chunks of one input reach the device. fill (may be empty): on a reader thread, once chunk ci of the plan is in
+// its ring slot. push: on the shard's thread, scores chunk ci and appends its records to sh.rec as file offsets; false
+// when the chunk is not the layout the device parses (the host parser then reads the whole input). `guess` is the
+// shard's own scratch, 0 before its first chunk.
+struct ChunkPush {
+    std::function<void(size_t ci, const char *slot)> fill;
+    std::function<bool(Shard &sh, size_t ci, const char *slot, size_t &guess)> push;
+};
+
+// FASTQ / FASTA text: the device finds the records (fl_reads_push_text)
+ChunkPush text_push(const std::vector<Chunk> &plan, int format) {
+    ChunkPush p;
+    p.push = [&plan, format](Shard &sh, size_t ci, const char *slot, size_t &guess) {
+        const Chunk &c = plan[ci];
+        const uint64_t nb = c.end - c.begin;
+        const bool last = ci + 1 == plan.size();
+        if (guess == 0) guess = (size_t)(nb / 256) + 1024;
+        for (;;) {
+            Records &R = sh.rec;
+            R.ensure(R.n + guess);
+            fl_text_records out{};
+            out.cap = guess;
+            out.name_off = R.name_off.data() + R.n; out.name_len = R.name_len.data() + R.n; out.comment_len = R.comment_len.data() + R.n;
+            out.seq_off = R.seq_off.data() + R.n; out.qual_off = R.qual_off.data() + R.n; out.len = R.len.data() + R.n;
+            out.name_hash = R.name_hash.data() + R.n;
+            uint64_t n_rec = 0, used = 0;
+            int status = 0;
+            const int rc = fl_reads_push_text(sh.ctx, slot, nb, format, last ? 1 : 0, &out, &n_rec, &used, &status);
+            if (rc == FL_ERANGE && n_rec > guess) { guess = (size_t)n_rec + 16; continue; }
+            check(sh.ctx, rc, "fl_reads_push_text");
+            if (status != FL_TEXT_OK || used != nb) return false;
+            for (size_t j = R.n; j < R.n + n_rec; ++j) {            // chunk offsets -> file offsets
+                R.name_off[j] += c.begin; R.seq_off[j] += c.begin; R.qual_off[j] += c.begin;
+            }
+            R.n += (size_t)n_rec;
+            guess = (size_t)n_rec + (size_t)n_rec / 4 + 1024;
+            return true;
+        }
+    };
+    return p;
+}
+
+// BAM: a reader thread checks and indexes the chunk's records (bam.h) while the shard's thread pushes the one before;
+// the device only gathers and scores (fl_reads_push_bam)
+ChunkPush bam_push(const char *base, const std::vector<Chunk> &plan, std::vector<BamChunkIndex> &idx) {
+    ChunkPush p;
+    p.fill = [base, &plan, &idx](size_t ci, const char *) { bam_index_chunk(base, plan[ci], idx[ci]); };
+    p.push = [&plan, &idx](Shard &sh, size_t ci, const char *slot, size_t &) {
+        BamChunkIndex &ix = idx[ci];
+        if (!ix.error.empty()) throw InputError(ix.error);
+        const Chunk &c = plan[ci];
+        const Records &X = ix.rec;
+        check(sh.ctx, fl_reads_push_bam(sh.ctx, slot, c.end - c.begin, X.n, ix.seq32.data(), ix.qual32.data(), X.len.data()),
+              "fl_reads_push_bam");
+        Records &R = sh.rec;
+        R.ensure(R.n + X.n);
+        for (size_t j = 0; j < X.n; ++j, ++R.n) {                   // chunk offsets -> file offsets
+            R.name_off[R.n] = X.name_off[j] + c.begin; R.seq_off[R.n] = X.seq_off[j] + c.begin; R.qual_off[R.n] = X.qual_off[j] + c.begin;
+            R.name_len[R.n] = X.name_len[j]; R.comment_len[R.n] = 0; R.len[R.n] = X.len[j]; R.name_hash[R.n] = X.name_hash[j];
+        }
+        ix = BamChunkIndex();
+        return true;
+    };
+    return p;
+}
+
 // get_ctx0: the caller's context for shard 0 (creating it may take the second or so the CUDA driver needs: the
 // readers below are already filling the ring by then)
-void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, int format, const fl_params &params, int nranks,
+void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, const ChunkPush &push, const fl_params &params, int nranks,
                const unsigned char *comm_id, const std::function<fl_ctx *()> &get_ctx0, std::atomic<bool> &abort_all, uint64_t slot_bytes,
                bool share_kmers) {
     Ring ring;
@@ -104,8 +178,8 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, i
                 for (size_t i = (size_t)k; i < n_chunks; i += ring.K) {
                     {
                         std::unique_lock<std::mutex> lk(ring.m);
-                        ring.cv.wait(lk, [&] { return ring.state[k] == 0 || abort_all.load(); });
-                        if (abort_all.load()) return;
+                        ring.cv.wait(lk, [&] { return ring.state[k] == 0 || abort_all.load() || ring.stop; });
+                        if (abort_all.load() || ring.stop) return;
                     }
                     const Chunk &c = plan[sh.chunk_lo + i];
                     uint64_t done = 0;
@@ -120,6 +194,7 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, i
                         if (r <= 0) { ok = false; break; }
                         done += (uint64_t)r;
                     }
+                    if (ok && push.fill) push.fill(sh.chunk_lo + i, ring.slot[k]);
                     {
                         std::lock_guard<std::mutex> lk(ring.m);
                         ring.state[k] = ok ? 1 : -1;
@@ -143,7 +218,7 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, i
                 check(sh.ctx, fl_kmers_finalize(sh.ctx, &nk), "fl_kmers_finalize");
             }
         }
-        size_t guess = 1024;
+        size_t guess = 0;
         for (size_t i = 0; i < n_chunks && !abort_all.load(); ++i) {
             const int k = (int)(i % ring.K);
             {
@@ -152,37 +227,17 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, i
                 if (abort_all.load()) break;
                 if (ring.state[k] < 0) throw std::runtime_error("Error reading the input file");
             }
-            const Chunk &c = plan[sh.chunk_lo + i];
-            const uint64_t nb = c.end - c.begin;
-            const bool last = sh.chunk_lo + i + 1 == plan.size();
-            if (i == 0) guess = (size_t)(nb / 256) + 1024;
-            for (;;) {
-                Records &R = sh.rec;
-                R.ensure(R.n + guess);
-                fl_text_records out{};
-                out.cap = guess;
-                out.name_off = R.name_off.data() + R.n; out.name_len = R.name_len.data() + R.n; out.comment_len = R.comment_len.data() + R.n;
-                out.seq_off = R.seq_off.data() + R.n; out.qual_off = R.qual_off.data() + R.n; out.len = R.len.data() + R.n;
-                out.name_hash = R.name_hash.data() + R.n;
-                uint64_t n_rec = 0, used = 0;
-                int status = 0;
-                const int rc = fl_reads_push_text(sh.ctx, ring.slot[k], nb, format, last ? 1 : 0, &out, &n_rec, &used, &status);
-                if (rc == FL_ERANGE && n_rec > guess) { guess = (size_t)n_rec + 16; continue; }
-                check(sh.ctx, rc, "fl_reads_push_text");
-                if (status != FL_TEXT_OK || used != nb) { sh.fallback = true; abort_all.store(true); break; }
-                for (size_t j = R.n; j < R.n + n_rec; ++j) {            // chunk offsets -> file offsets
-                    R.name_off[j] += c.begin; R.seq_off[j] += c.begin; R.qual_off[j] += c.begin;
-                }
-                R.n += (size_t)n_rec;
-                guess = (size_t)n_rec + (size_t)n_rec / 4 + 1024;
-                break;
-            }
+            if (!push.push(sh, sh.chunk_lo + i, ring.slot[k], guess)) { sh.fallback = true; abort_all.store(true); break; }
             {
                 std::lock_guard<std::mutex> lk(ring.m);
                 ring.state[k] = 0;
             }
             ring.cv.notify_all();
         }
+    } catch (const InputError &e) {
+        sh.error = e.what();
+        std::lock_guard<std::mutex> lk(ring.m);
+        ring.stop = true;
     } catch (const std::exception &e) {
         sh.error = e.what();
         abort_all.store(true);
@@ -253,24 +308,42 @@ bool find_duplicate(const std::vector<Shard> &shards, const char *base, std::str
 
 FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function<void(const char *)> &mark) {
     FeederOutcome res;
-    if (args.verbose || getenv("FL_HOST_PARSER")) return res;           // per-read dumps come from the host path
+    // per-read dumps come from the host path, which reads text only: a BAM input always takes this one
+    const bool host_parser = args.verbose || getenv("FL_HOST_PARSER");
+    if (host_parser && !bam_file_magic(args.input_reads)) return res;
     MappedFile f;
     bool inflated = false;
-    if (!f.open_any(args.input_reads, &inflated)) return res;           // neither plain nor gzip that fits in memory: the host reader
+    std::string why;
+    if (!f.open_any(args.input_reads, &inflated, &why)) {               // neither plain nor gzip that fits in memory: the host reader
+        if (f.gzip && bam_file_magic(args.input_reads)) throw std::runtime_error("cannot read BAM input " + args.input_reads + ": " + why);
+        return res;
+    }
     if (inflated) mark("gzip input inflated into memory");
     const int format = f.format();
     if (!format) return res;
+    const bool bam = format == FL_FORMAT_BAM;
+    if (bam && args.verbose) throw std::runtime_error("--verbose is not supported with BAM input");
+    if (!bam && host_parser) return res;
     const bool kmers_empty = kmers.empty();
     if (format == FL_TEXT_FASTA && kmers_empty) return res;             // main.cpp:103-106: the host path prints the error
     uint64_t target = 128ull << 20;
     if (const char *e = getenv("FL_CHUNK_MB")) target = (uint64_t)atoll(e) << 20;
     if (target < (1ull << 20)) target = 1ull << 20;
     if (target > (1024ull << 20)) target = 1024ull << 20;
-    const uint64_t max_chunk = target;                                   // plan_chunks never cuts later than `target` bytes after a chunk's start
+    uint64_t max_chunk = target;                                         // plan_chunks never cuts later than `target` bytes after a chunk's start
     int nranks = args.gpus;
     std::vector<Chunk> plan;
-    if (!plan_chunks(f.base, f.size, format, target, max_chunk, plan) || plan.empty()) return res;
-    if ((size_t)nranks > plan.size()) nranks = (int)plan.size();         // tiny inputs: fewer shards than GPUs asked for
+    uint64_t bam_header_bytes = 0;
+    if (bam) {                                                           // a BAM file's records are known here or never: no host reader
+        if (!bam_header(f.base, f.size, &bam_header_bytes, &why) || !bam_plan_chunks(f.base, f.size, bam_header_bytes, target, plan, &max_chunk, &why))
+            throw std::runtime_error(why);
+        mark("BAM block_size chain");
+    } else if (!plan_chunks(f.base, f.size, format, target, max_chunk, plan) || plan.empty()) {
+        return res;
+    }
+    if ((size_t)nranks > plan.size()) nranks = plan.empty() ? 1 : (int)plan.size();   // tiny inputs: fewer shards than GPUs asked for
+    std::vector<BamChunkIndex> bam_idx(bam ? plan.size() : 0);
+    const ChunkPush push = bam ? bam_push(f.base, plan, bam_idx) : text_push(plan, format);
 
     const fl_params params = params_from_arguments(args);
     unsigned char comm_id[FL_COMM_ID_BYTES] = {0};
@@ -298,9 +371,9 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
     {
         std::vector<std::thread> ts;
         for (int r = 1; r < nranks; ++r)
-            ts.emplace_back(run_shard, std::ref(shards[r]), std::cref(f), std::cref(plan), format, std::cref(params), nranks, comm_id,
+            ts.emplace_back(run_shard, std::ref(shards[r]), std::cref(f), std::cref(plan), std::cref(push), std::cref(params), nranks, comm_id,
                             std::cref(get_ctx0), std::ref(abort_all), max_chunk, !kmers_empty);
-        run_shard(shards[0], f, plan, format, params, nranks, comm_id, get_ctx0, abort_all, max_chunk, !kmers_empty);
+        run_shard(shards[0], f, plan, push, params, nranks, comm_id, get_ctx0, abort_all, max_chunk, !kmers_empty);
         for (auto &t : ts) t.join();
     }
     auto cleanup = [&]() {
@@ -317,13 +390,40 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
         guard.release();
         return res;
     }
-    mark("pass 1 (device parse + score)");
+    mark(bam ? "pass 1 (BAM records + score)" : "pass 1 (device parse + score)");
     res.handled = true;
     std::cerr << "Scoring long reads\n";
     long long n_reads = 0, total_bases = 0;
     for (auto &s : shards) {
         n_reads += (long long)s.rec.n;
         for (size_t i = 0; i < s.rec.n; ++i) total_bases += s.rec.len[i];
+    }
+    if (bam) {
+        // the checks main.cpp:77-106 makes of the FASTQ equivalent, whose FASTA records are those without quality
+        const Records *first_q = nullptr, *first_f = nullptr;
+        size_t iq = 0, i_f = 0;
+        long long nq = -1, nf = -1, k = 0;
+        for (auto &s : shards)
+            for (size_t i = 0; i < s.rec.n && (nq < 0 || nf < 0); ++i, ++k) {
+                const bool fasta = bam_no_quality(f.base + s.rec.qual_off[i]);
+                if (fasta && nf < 0) { nf = k; first_f = &s.rec; i_f = i; }
+                if (!fasta && nq < 0) { nq = k; first_q = &s.rec; iq = i; }
+            }
+        const char *error = nullptr;
+        const Records *at = nullptr;
+        size_t ai = 0;
+        if (nf >= 0 && kmers_empty && (nq < 0 || nf < nq)) error = "FASTA input not supported without an external reference";
+        else if (nf >= 0 && nq >= 0) {
+            error = "could not parse input reads";
+            if (nf > nq) { at = first_f; ai = i_f; } else { at = first_q; ai = iq; }
+        }
+        if (error) {
+            std::cerr << "\n\n" << "Error: " << error << "\n";
+            if (at) std::cerr << "  problem occurred at read " << std::string(f.base + at->name_off[ai], at->name_len[ai]) << "\n";
+            cleanup();
+            res.exit_code = 1;
+            return res;
+        }
     }
     {
         std::string dup;
@@ -356,8 +456,9 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
     std::cerr << "Outputting passed long reads\n";
     std::vector<Part> parts;
     for (auto &s : shards) parts.push_back(Part{&s.rec, Results::of(s)});
-    const Format fmt{format == FL_TEXT_FASTA ? '>' : '@', format == FL_TEXT_FASTQ};
-    const bool out_failed = !write_survivors(g_out_fd, f.base, parts, fmt, args.bgzip ? ctx0 : nullptr);
+    const Format fmt{format == FL_TEXT_FASTA ? '>' : '@', format == FL_TEXT_FASTQ, bam, bam_header_bytes};
+    // BAM in, BAM out: always BGZF (--bgzip changes nothing)
+    const bool out_failed = !write_survivors(g_out_fd, f.base, parts, fmt, args.bgzip || bam ? ctx0 : nullptr);
     mark("pass 2 (slices of the mapped input)");
     std::cerr << "\n";
     cleanup();

@@ -13,6 +13,9 @@
 //   * pass 2 writes the survivors straight from the mapping (survivors.h: writev, or pwrite groups into a regular file).
 //   * a gzip file is inflated ONCE into memory (gzmem.h: BGZF blocks by several host threads, anything else by one)
 //     and then goes down the same path; the reference inflates it once per pass.
+//   * an unaligned BAM file (bam.h) is inflated the same way; the reader threads check and index its records, the device
+//     gathers and scores them (fl_reads_push_bam) and pass 2 writes BAM. It always takes this path: its errors are
+//     thrown from here (nothing reaches stdout), and --verbose with it is one of them.
 // Anything else -- CR LF, multi-line records, broken records, a gzip file that is damaged or would not fit in memory,
 // --verbose -- makes run_text_feeder return handled == false before anything was printed to stdout, and main() runs
 // the kseq-compatible host parser.

@@ -101,7 +101,7 @@ int Kmers::add_reference(const std::string &filename, bool multi) {
     MappedFile f;
     std::vector<Chunk> plan;
     const bool timing = getenv("FL_CLI_TIMING") != nullptr;
-    bool text_path = !getenv("FL_HOST_PARSER") && f.open_any(filename) && f.format() != 0;
+    bool text_path = !getenv("FL_HOST_PARSER") && f.open_any(filename) && (f.format() == FL_TEXT_FASTQ || f.format() == FL_TEXT_FASTA);
     if (text_path) {
         // a chunk holds whole records: FASTA chunks are large enough for a chromosome on one line or wrapped
         uint64_t target = f.format() == FL_TEXT_FASTA ? 512ull << 20 : 128ull << 20;

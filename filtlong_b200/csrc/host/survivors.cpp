@@ -13,6 +13,7 @@
 #include <iostream>
 #include <thread>
 
+#include "bam.h"
 #include "bgzf_out.h"
 #include "fastx.h"
 #include "misc.h"
@@ -58,6 +59,22 @@ size_t c_substr(size_t n, size_t start, size_t length) { return start >= n ? 0 :
 // must stay valid until the sink is flushed; put_owned() keeps its string alive until then.
 template <class Sink>
 void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Results &res, size_t i) {
+    if (fmt.bam) {                                                        // the record as it is, or new ones for the children
+        const char *rec = bam_record_of(r.name);
+        const size_t rs = (size_t)res.row_start[i];
+        if (res.n_child[i] == 0) {
+            if (res.row_pfinal[rs]) sink.put(rec, bam_record_bytes(rec));
+            return;
+        }
+        for (size_t row = rs; row < rs + (size_t)res.n_child[i]; ++row) {
+            const int start = res.row_s[row], end = res.row_e[row];
+            if (!res.row_pfinal[row] || end - start <= 0 || (size_t)end > r.len) continue;
+            std::string child;
+            bam_child_record(rec, start, end, child);
+            sink.put_owned(std::move(child));
+        }
+        return;
+    }
     const char *lead = fmt.lead == '>' ? ">" : "@";
     auto rest = [&](size_t start, size_t length) {
         if (r.has_comment) { sink.put(" ", 1); sink.put(r.comment, r.comment_print); }
@@ -213,8 +230,16 @@ bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, c
     if (bgzf) {
         // compressed offsets are not known in advance: pipe or file, the members are written in order
         BgzfOut z(bgzf, fd);
+        if (fmt.bam) z.put(base, (size_t)fmt.bam_header);
         for (const Part &p : parts) emit_range(z, base, p, 0, p.rec->n, fmt);
         return finish(z);
+    }
+    if (fmt.bam) {
+        Copier c(fd, -1);
+        c.put(base, (size_t)fmt.bam_header);
+        for (const Part &p : parts) emit_range(c, base, p, 0, p.rec->n, fmt);
+        c.flush();
+        return !c.failed;
     }
     struct stat st;
     const int flags = fcntl(fd, F_GETFL);

@@ -1,7 +1,7 @@
 // filtlong_b200/csrc/host/survivors.h -- pass 2 of the CLI: the surviving reads and child rows in input order, as the
 // reference prints them (reference src/main.cpp:263-313), and the stderr blocks that lead up to it. The only code that
 // knows that output layout and how the bytes reach the descriptor. Two sources feed it:
-//   * random access: the mapped input and a table of where each record sits (the device feeder's, one part per shard, or
+//   * random access: the mapped input (or an inflated BAM file) and a table of where each record sits (the device feeder's, one part per shard, or
 //     the host reader's when every record was simple). To BGZF; to pwrite() groups written by a few threads when the
 //     descriptor is a regular file not opened with O_APPEND; else to writev().
 //   * sequential: the input parsed again by FastxReader (streamed gzip, CR LF, multi-line records), copied through a
@@ -52,6 +52,8 @@ struct Results {
 struct Format {
     char lead;                    // '>' or '@'
     bool quality;                 // print "+" and the quality
+    bool bam = false;             // BAM records (bam.h) instead of text; then lead and quality are not used
+    uint64_t bam_header = 0;      // BAM: bytes [0, bam_header) of the input are the header, written first
 };
 
 struct Part {                     // one part of the table, with its results
@@ -69,7 +71,9 @@ inline void append_child_name(std::string &out, const char *name, size_t name_le
 }
 
 // Random access: the survivors of `parts`, in order, from the input mapped at `base`; compressed on the context `bgzf`
-// when it is given. The last two are the choices write_survivors makes, callable directly.
+// when it is given. The last two are the choices write_survivors makes, callable directly. BAM (fmt.bam): the header,
+// then each kept read's record as it is and a new record for each kept child; the CLI always passes a context, without
+// one the uncompressed BAM stream is written.
 bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf);
 bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);
 bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);

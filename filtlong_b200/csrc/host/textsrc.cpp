@@ -8,6 +8,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include "bam.h"
 #include "gzmem.h"
 
 bool MappedFile::open_plain(const std::string &path) {
@@ -40,13 +41,23 @@ bool MappedFile::inflate(std::string *why) {
     return true;
 }
 
-bool MappedFile::open_any(const std::string &path, bool *inflated) {
+bool MappedFile::open_any(const std::string &path, bool *inflated, std::string *why) {
     if (inflated) *inflated = false;
     if (open_plain(path)) return true;
-    std::string why;
-    if (!gzip || getenv("FL_GZ_HOST") || !inflate(&why)) return false;   // not gzip either, or declined (gzmem.h)
+    std::string w;
+    if (!why) why = &w;
+    if (!gzip) return false;                                           // not gzip either
+    if (getenv("FL_GZ_HOST")) { *why = "FL_GZ_HOST is set"; return false; }
+    if (!inflate(why)) return false;                                   // declined (gzmem.h)
     if (inflated) *inflated = true;
     return true;
+}
+
+int MappedFile::format() const {
+    if (!base || !size) return 0;
+    if (base[0] == '@') return FL_TEXT_FASTQ;
+    if (base[0] == '>') return FL_TEXT_FASTA;
+    return fd < 0 && bam_magic(base, size) ? FL_FORMAT_BAM : 0;
 }
 
 MappedFile::~MappedFile() {

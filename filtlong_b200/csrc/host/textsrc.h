@@ -19,9 +19,11 @@ struct MappedFile {
     // gzip: inflate the whole file ONCE into memory (gzmem.h) and carry on as if it were a mapped plain file; the
     // reference inflates it once per pass (main.cpp:70-75, 263-269). false: leave it to the host reader.
     bool inflate(std::string *why);
-    // plain file, or gzip inflated into memory (unless FL_GZ_HOST is set); false: use the streaming host reader
-    bool open_any(const std::string &path, bool *inflated = nullptr);
-    int format() const { return !base || !size ? 0 : (base[0] == '@' ? FL_TEXT_FASTQ : (base[0] == '>' ? FL_TEXT_FASTA : 0)); }
+    // plain file, or gzip inflated into memory (unless FL_GZ_HOST is set); false: use the streaming host reader (*why:
+    // why a gzip file was not inflated)
+    bool open_any(const std::string &path, bool *inflated = nullptr, std::string *why = nullptr);
+    // FL_TEXT_FASTQ, FL_TEXT_FASTA, FL_FORMAT_BAM (bam.h: an inflated input that starts with the BAM magic), or 0
+    int format() const;
     MappedFile() = default;
     MappedFile(const MappedFile &) = delete;
     MappedFile &operator=(const MappedFile &) = delete;

@@ -193,6 +193,14 @@ typedef struct fl_text_records {
 } fl_text_records;
 int fl_reads_push_text(fl_ctx *ctx, const char *host_text, uint64_t n_bytes, int format, int is_last_chunk,
                        const fl_text_records *out, uint64_t *n_records, uint64_t *bytes_consumed, int *status);
+/* Unaligned BAM input: a chunk of inflated BAM bytes holding n_rec whole records, and per record where its SEQ
+ * (seq_off, 4-bit codes) and QUAL (qual_off) start, relative to the chunk, and its length (l_seq >= 1). The caller has
+ * walked and checked the records (host/bam.cpp). Each record is scored as the record of its FASTQ equivalent: in Phred
+ * mode the quality is QUAL + 33, in k-mer mode the sequence is SEQ decoded with "=ACMGRSVTWYHKDBN". Same buffer-reuse
+ * rules as fl_reads_push_text: the chunk and the arrays may be reused when the call returns. FL_EINVAL if a record does
+ * not lie inside the chunk. */
+int fl_reads_push_bam(fl_ctx *ctx, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
+                      const uint32_t *qual_off, const int32_t *len);
 /* The reference set from a chunk of the reference FILE (replaces the kseq_read loop of Kmers::add_reference,
  * kmers.cpp:75-134, for the common layouts): same contract as fl_reads_push_text -- the chunk starts at a record boundary,
  * LF line ends, FL_TEXT_FALLBACK and nothing added otherwise -- but the records' sequences go to the 16-mer set like
