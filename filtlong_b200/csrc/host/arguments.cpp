@@ -10,6 +10,11 @@
 #include <sstream>
 #include <stdexcept>
 
+#include <sys/stat.h>
+#include <unistd.h>
+
+#include "streamsrc.h"
+
 namespace {
 
 struct ParseError : std::runtime_error {
@@ -108,7 +113,7 @@ void print_help(const char *prog) {
     std::ostream &o = std::cerr;
     o << "usage: " << prog << " {OPTIONS} [input_reads]\n\n"
       << "Filtlong: a quality filtering tool for Nanopore and PacBio reads\n\n"
-      << "positional arguments:\n   input_reads                          input long reads to be filtered\n\n";
+      << "positional arguments:\n   input_reads                          input long reads to be filtered (- for standard input)\n\n";
     struct Group { const char *title; int first, last; };
     const Group groups[] = {
         {"output thresholds:", 0, 5},
@@ -229,7 +234,8 @@ Arguments::Arguments(int argc, char **argv) {
     const bool some_reference = !short_reads.empty() || assembly_set;
     if (trim && !some_reference) FAIL("Error: assembly or read reference is required to use --trim");
     if (split_set && !some_reference) FAIL("Error: assembly or read reference is required to use --split");
-    std::vector<std::string> files{input_reads};
+    if (!reads_exist(input_reads)) FAIL("Error: cannot find file: " + input_reads);
+    std::vector<std::string> files;
     for (const auto &f : short_reads) files.push_back(f);
     if (assembly_set) files.push_back(assembly);
     for (const auto &f : files)
@@ -254,4 +260,13 @@ Arguments::Arguments(int argc, char **argv) {
 bool Arguments::does_file_exist(const std::string &filename) {
     std::ifstream infile(filename);
     return infile.good();
+}
+
+// The input reads may also be a stream (streamsrc.h): "-" is standard input, and a FIFO, a character device or a socket
+// is checked without being opened (opening and closing a FIFO would cost its writer the data it has written).
+bool Arguments::reads_exist(const std::string &filename) {
+    struct stat st;
+    if (filename == "-") return fstat(0, &st) == 0;
+    if (is_stream_file(filename)) return access(filename.c_str(), R_OK) == 0;
+    return does_file_exist(filename);
 }

@@ -47,4 +47,5 @@ public:
 
 private:
     bool does_file_exist(const std::string &filename);
+    bool reads_exist(const std::string &filename);
 };

@@ -40,8 +40,8 @@ public:
     // must not be used.
     bool simple = false;
     uint64_t name_off = 0, comment_off = 0, seq_off = 0, qual_off = 0;
-    // true when the file is not compressed: stream offsets are file offsets
-    bool plain() const { return fp_ && gzdirect(fp_) != 0; }
+    // true when the offsets are those of the bytes given: a file that is not compressed, or memory
+    bool plain() const { return mem_ != nullptr || (fp_ && gzdirect(fp_) != 0); }
 
 private:
     int getc();

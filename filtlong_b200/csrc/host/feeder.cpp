@@ -6,6 +6,7 @@
 
 #include <stdlib.h>
 
+#include <algorithm>
 #include <atomic>
 #include <condition_variable>
 #include <iostream>
@@ -18,6 +19,7 @@
 #include "bam.h"
 #include "misc.h"
 #include "read.h"
+#include "streamsrc.h"
 #include "survivors.h"
 #include "textsrc.h"
 
@@ -87,22 +89,64 @@ struct InputError : std::runtime_error {
     using std::runtime_error::runtime_error;
 };
 
-// How the chunks of one input reach the device. fill (may be empty): on a reader thread, once chunk ci of the plan is in
-// its ring slot. push: on the shard's thread, scores chunk ci and appends its records to sh.rec as file offsets; false
-// when the chunk is not the layout the device parses (the host parser then reads the whole input). `guess` is the
+// The chunks of the input, in order. A file's plan is whole before the first push (done()); a stream's grows while the
+// stream arrives (add(), then close()), and the shard's readers and pusher wait for the chunks they need.
+class Plan {
+public:
+    std::vector<Chunk> chunks;              // a whole plan: set before any shard runs, read-only afterwards
+    void done() { complete_ = true; }
+    // `final`: c is the input's last chunk (the plan is complete with it, in the same step)
+    void add(const Chunk &c, bool final) {
+        {
+            std::lock_guard<std::mutex> lk(m_);
+            chunks.push_back(c);
+            complete_ = complete_ || final;
+        }
+        cv_.notify_all();
+    }
+    bool failed() {
+        std::lock_guard<std::mutex> lk(m_);
+        return failed_;
+    }
+    // ok == false: no boundary to cut at, or the stream broke; or cancel(): a shard stopped
+    void close(bool ok) {
+        { std::lock_guard<std::mutex> lk(m_); complete_ = true; failed_ = failed_ || !ok; }
+        cv_.notify_all();
+    }
+    void cancel() { close(false); }
+    // Chunk i and whether it is the input's last. 1: *c, *last set; 0: the plan ended before chunk i; -1: it failed first.
+    // A chunk cut while the stream still arrives is never the last: bytes after it have arrived.
+    int get(size_t i, Chunk *c, bool *last) {
+        std::unique_lock<std::mutex> lk(m_);
+        cv_.wait(lk, [&] { return i < chunks.size() || complete_; });
+        if (i < chunks.size() && !failed_) {
+            *c = chunks[i];
+            *last = complete_ && i + 1 == chunks.size();
+            return 1;
+        }
+        return failed_ ? -1 : 0;
+    }
+
+private:
+    std::mutex m_;
+    std::condition_variable cv_;
+    bool complete_ = false, failed_ = false;
+};
+
+// How the chunks of one input reach the device. fill (may be empty): on a reader thread, once chunk ci (c) of the plan
+// is in its ring slot. push: on the shard's thread, scores chunk ci and appends its records to sh.rec as file offsets;
+// false when the chunk is not the layout the device parses (the host parser then reads the whole input). `guess` is the
 // shard's own scratch, 0 before its first chunk.
 struct ChunkPush {
-    std::function<void(size_t ci, const char *slot)> fill;
-    std::function<bool(Shard &sh, size_t ci, const char *slot, size_t &guess)> push;
+    std::function<void(size_t ci, const Chunk &c, const char *slot)> fill;
+    std::function<bool(Shard &sh, size_t ci, const Chunk &c, bool last, const char *slot, size_t &guess)> push;
 };
 
 // FASTQ / FASTA text: the device finds the records (fl_reads_push_text)
-ChunkPush text_push(const std::vector<Chunk> &plan, int format) {
+ChunkPush text_push(int format) {
     ChunkPush p;
-    p.push = [&plan, format](Shard &sh, size_t ci, const char *slot, size_t &guess) {
-        const Chunk &c = plan[ci];
+    p.push = [format](Shard &sh, size_t, const Chunk &c, bool last, const char *slot, size_t &guess) {
         const uint64_t nb = c.end - c.begin;
-        const bool last = ci + 1 == plan.size();
         if (guess == 0) guess = (size_t)(nb / 256) + 1024;
         for (;;) {
             Records &R = sh.rec;
@@ -131,13 +175,12 @@ ChunkPush text_push(const std::vector<Chunk> &plan, int format) {
 
 // BAM: a reader thread checks and indexes the chunk's records (bam.h) while the shard's thread pushes the one before;
 // the device only gathers and scores (fl_reads_push_bam)
-ChunkPush bam_push(const char *base, const std::vector<Chunk> &plan, std::vector<BamChunkIndex> &idx) {
+ChunkPush bam_push(const char *base, std::vector<BamChunkIndex> &idx) {
     ChunkPush p;
-    p.fill = [base, &plan, &idx](size_t ci, const char *) { bam_index_chunk(base, plan[ci], idx[ci]); };
-    p.push = [&plan, &idx](Shard &sh, size_t ci, const char *slot, size_t &) {
+    p.fill = [base, &idx](size_t ci, const Chunk &c, const char *) { bam_index_chunk(base, c, idx[ci]); };
+    p.push = [&idx](Shard &sh, size_t ci, const Chunk &c, bool, const char *slot, size_t &) {
         BamChunkIndex &ix = idx[ci];
         if (!ix.error.empty()) throw InputError(ix.error);
-        const Chunk &c = plan[ci];
         const Records &X = ix.rec;
         check(sh.ctx, fl_reads_push_bam(sh.ctx, slot, c.end - c.begin, X.n, ix.seq32.data(), ix.qual32.data(), X.len.data()),
               "fl_reads_push_bam");
@@ -155,9 +198,9 @@ ChunkPush bam_push(const char *base, const std::vector<Chunk> &plan, std::vector
 
 // get_ctx0: the caller's context for shard 0 (creating it may take the second or so the CUDA driver needs: the
 // readers below are already filling the ring by then)
-void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, const ChunkPush &push, const fl_params &params, int nranks,
+void run_shard(Shard &sh, const MappedFile &f, Plan &plan, const ChunkPush &push, const fl_params &params, int nranks,
                const unsigned char *comm_id, const std::function<fl_ctx *()> &get_ctx0, std::atomic<bool> &abort_all, uint64_t slot_bytes,
-               bool share_kmers) {
+               bool share_kmers, StreamInput *stream) {
     Ring ring;
     if (const char *e = getenv("FL_READERS")) {
         const int k = atoi(e);
@@ -181,11 +224,13 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, c
                         ring.cv.wait(lk, [&] { return ring.state[k] == 0 || abort_all.load() || ring.stop; });
                         if (abort_all.load() || ring.stop) return;
                     }
-                    const Chunk &c = plan[sh.chunk_lo + i];
+                    Chunk c;
+                    bool last;
+                    if (plan.get(sh.chunk_lo + i, &c, &last) != 1) return;    // a stream's plan ended (the pusher sees it too)
                     uint64_t done = 0;
                     const uint64_t want = c.end - c.begin;
                     bool ok = true;
-                    if (f.fd < 0) {                                    // inflated gzip input: already in memory
+                    if (f.fd < 0) {                                    // inflated gzip input or a stream: already in memory
                         memcpy(ring.slot[k], f.base + c.begin, (size_t)want);
                         done = want;
                     }
@@ -194,7 +239,7 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, c
                         if (r <= 0) { ok = false; break; }
                         done += (uint64_t)r;
                     }
-                    if (ok && push.fill) push.fill(sh.chunk_lo + i, ring.slot[k]);
+                    if (ok && push.fill) push.fill(sh.chunk_lo + i, c, ring.slot[k]);
                     {
                         std::lock_guard<std::mutex> lk(ring.m);
                         ring.state[k] = ok ? 1 : -1;
@@ -221,13 +266,22 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, c
         size_t guess = 0;
         for (size_t i = 0; i < n_chunks && !abort_all.load(); ++i) {
             const int k = (int)(i % ring.K);
+            Chunk c;
+            bool last;
+            const int got = plan.get(sh.chunk_lo + i, &c, &last);
+            if (got == 0) break;                                       // the end of a stream
+            if (got < 0) { sh.fallback = true; abort_all.store(true); break; }
             {
                 std::unique_lock<std::mutex> lk(ring.m);
                 ring.cv.wait(lk, [&] { return ring.state[k] != 0 || abort_all.load(); });
                 if (abort_all.load()) break;
                 if (ring.state[k] < 0) throw std::runtime_error("Error reading the input file");
             }
-            if (!push.push(sh, sh.chunk_lo + i, ring.slot[k], guess)) { sh.fallback = true; abort_all.store(true); break; }
+            if (!push.push(sh, sh.chunk_lo + i, c, last, ring.slot[k], guess)) { sh.fallback = true; abort_all.store(true); break; }
+            if (stream) {
+                ++stream->chunks;
+                if (!stream->ended()) ++stream->chunks_before_end;
+            }
             {
                 std::lock_guard<std::mutex> lk(ring.m);
                 ring.state[k] = 0;
@@ -242,6 +296,7 @@ void run_shard(Shard &sh, const MappedFile &f, const std::vector<Chunk> &plan, c
         sh.error = e.what();
         abort_all.store(true);
     }
+    if (abort_all.load()) plan.cancel();                               // readers waiting for a stream's next chunk
     ring.cv.notify_all();
     for (auto &t : readers) t.join();
     for (int k = 0; k < ring.K; ++k) {
@@ -306,20 +361,41 @@ bool find_duplicate(const std::vector<Shard> &shards, const char *base, std::str
 
 }  // namespace
 
-FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function<void(const char *)> &mark) {
+FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, StreamInput *stream, const std::function<void(const char *)> &mark) {
     FeederOutcome res;
     // per-read dumps come from the host path, which reads text only: a BAM input always takes this one
     const bool host_parser = args.verbose || getenv("FL_HOST_PARSER");
-    if (host_parser && !bam_file_magic(args.input_reads)) return res;
-    MappedFile f;
-    bool inflated = false;
+    MappedFile own;
+    const MappedFile *fp = &own;
     std::string why;
-    if (!f.open_any(args.input_reads, &inflated, &why)) {               // neither plain nor gzip that fits in memory: the host reader
-        if (f.gzip && bam_file_magic(args.input_reads)) throw std::runtime_error("cannot read BAM input " + args.input_reads + ": " + why);
-        return res;
+    int format = 0;
+    // a stream's plain text goes to the device while it arrives (one GPU); anything else is read to its end first
+    bool growing = false;
+    if (stream) {
+        bool ended = false;
+        const uint64_t head = stream->wait_for(2, &ended);
+        const char b0 = head ? stream->base()[0] : 0;
+        growing = !host_parser && args.gpus == 1 && head >= 2 && (b0 == '@' || b0 == '>');
+        if (growing) format = b0 == '@' ? FL_TEXT_FASTQ : FL_TEXT_FASTA;
+        else if (!stream->finish(&why)) throw std::runtime_error(why);
+        fp = &stream->file();
+        if (stream->inflated()) mark("gzip input inflated into memory");
+        if (!growing) {
+            if (fp->size < 2 && !stream->inflated()) return res;        // as MappedFile::open_plain declines a file that small
+            format = fp->format();
+            if (host_parser && format != FL_FORMAT_BAM) return res;
+        }
+    } else {
+        if (host_parser && !bam_file_magic(args.input_reads)) return res;
+        bool inflated = false;
+        if (!own.open_any(args.input_reads, &inflated, &why)) {         // neither plain nor gzip that fits in memory: the host reader
+            if (own.gzip && bam_file_magic(args.input_reads)) throw std::runtime_error("cannot read BAM input " + args.input_reads + ": " + why);
+            return res;
+        }
+        if (inflated) mark("gzip input inflated into memory");
+        format = own.format();
     }
-    if (inflated) mark("gzip input inflated into memory");
-    const int format = f.format();
+    const MappedFile &f = *fp;
     if (!format) return res;
     const bool bam = format == FL_FORMAT_BAM;
     if (bam && args.verbose) throw std::runtime_error("--verbose is not supported with BAM input");
@@ -332,18 +408,23 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
     if (target > (1024ull << 20)) target = 1024ull << 20;
     uint64_t max_chunk = target;                                         // plan_chunks never cuts later than `target` bytes after a chunk's start
     int nranks = args.gpus;
-    std::vector<Chunk> plan;
+    Plan plan;
     uint64_t bam_header_bytes = 0;
-    if (bam) {                                                           // a BAM file's records are known here or never: no host reader
-        if (!bam_header(f.base, f.size, &bam_header_bytes, &why) || !bam_plan_chunks(f.base, f.size, bam_header_bytes, target, plan, &max_chunk, &why))
+    if (growing) {
+        // cut by the planner thread below
+    } else if (bam) {                                                    // a BAM file's records are known here or never: no host reader
+        if (!bam_header(f.base, f.size, &bam_header_bytes, &why) || !bam_plan_chunks(f.base, f.size, bam_header_bytes, target, plan.chunks, &max_chunk, &why))
             throw std::runtime_error(why);
         mark("BAM block_size chain");
-    } else if (!plan_chunks(f.base, f.size, format, target, max_chunk, plan) || plan.empty()) {
+    } else if (!plan_chunks(f.base, f.size, format, target, max_chunk, plan.chunks) || plan.chunks.empty()) {
         return res;
     }
-    if ((size_t)nranks > plan.size()) nranks = plan.empty() ? 1 : (int)plan.size();   // tiny inputs: fewer shards than GPUs asked for
-    std::vector<BamChunkIndex> bam_idx(bam ? plan.size() : 0);
-    const ChunkPush push = bam ? bam_push(f.base, plan, bam_idx) : text_push(plan, format);
+    if (!growing) {
+        plan.done();
+        if ((size_t)nranks > plan.chunks.size()) nranks = plan.chunks.empty() ? 1 : (int)plan.chunks.size();   // tiny inputs: fewer shards than GPUs asked for
+    }
+    std::vector<BamChunkIndex> bam_idx(bam ? plan.chunks.size() : 0);
+    const ChunkPush push = bam ? bam_push(f.base, bam_idx) : text_push(format);
 
     const fl_params params = params_from_arguments(args);
     unsigned char comm_id[FL_COMM_ID_BYTES] = {0};
@@ -360,21 +441,42 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
             shards[r].chunk_lo = c;
             shards[r].rec.lead_checked = true;
             const uint64_t goal = f.size / (uint64_t)nranks * (uint64_t)(r + 1);
-            while (c < plan.size() && (r + 1 == nranks || plan[c].end <= goal || c == shards[r].chunk_lo)) ++c;
+            const std::vector<Chunk> &cs = plan.chunks;
+            while (c < cs.size() && (r + 1 == nranks || cs[c].end <= goal || c == shards[r].chunk_lo)) ++c;
             shards[r].chunk_hi = c;
         }
-        shards.back().chunk_hi = plan.size();
+        shards.back().chunk_hi = growing ? SIZE_MAX : plan.chunks.size();
     }
     std::atomic<bool> abort_all(false);
     fl_ctx *ctx0 = nullptr;
     const std::function<fl_ctx *()> get_ctx0 = [&]() { ctx0 = kmers.context(); return ctx0; };
     {
+        // a stream's chunks are cut here as its bytes arrive, the same cuts plan_chunks makes of the whole (textsrc.h)
+        std::thread planner;
+        if (growing)
+            planner = std::thread([&] {
+                uint64_t pos = 0, avail = 0;
+                for (;;) {
+                    bool ended = false;
+                    avail = stream->wait_for(std::max(avail + 1, pos + target + 1), &ended);   // what plan_next_chunk needs to cut
+                    if (ended && stream->broken()) { plan.close(false); return; }
+                    Chunk c;
+                    int r;
+                    while ((r = plan_next_chunk(f.base, avail, ended, format, target, max_chunk, pos, &c)) == 1) {
+                        pos = c.end;
+                        plan.add(c, ended && pos == avail);
+                    }
+                    if (r < 0 || plan.failed()) { plan.close(false); return; }
+                    if (ended) { plan.close(true); return; }
+                }
+            });
         std::vector<std::thread> ts;
         for (int r = 1; r < nranks; ++r)
-            ts.emplace_back(run_shard, std::ref(shards[r]), std::cref(f), std::cref(plan), std::cref(push), std::cref(params), nranks, comm_id,
-                            std::cref(get_ctx0), std::ref(abort_all), max_chunk, !kmers_empty);
-        run_shard(shards[0], f, plan, push, params, nranks, comm_id, get_ctx0, abort_all, max_chunk, !kmers_empty);
+            ts.emplace_back(run_shard, std::ref(shards[r]), std::cref(f), std::ref(plan), std::cref(push), std::cref(params), nranks, comm_id,
+                            std::cref(get_ctx0), std::ref(abort_all), max_chunk, !kmers_empty, stream);
+        run_shard(shards[0], f, plan, push, params, nranks, comm_id, get_ctx0, abort_all, max_chunk, !kmers_empty, stream);
         for (auto &t : ts) t.join();
+        if (planner.joinable()) planner.join();
     }
     auto cleanup = [&]() {
         for (auto &s : shards) {
@@ -382,6 +484,7 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function
             if (s.owns_ctx && s.ctx) fl_ctx_destroy(s.ctx);
         }
     };
+    if (growing && !stream->finish(&why)) { cleanup(); throw std::runtime_error(why); }
     for (auto &s : shards)
         if (!s.error.empty()) { cleanup(); throw std::runtime_error(s.error); }
     if (abort_all.load()) {                                             // not the simple layout after all: start over on the host

@@ -16,18 +16,24 @@
 //   * an unaligned BAM file (bam.h) is inflated the same way; the reader threads check and index its records, the device
 //     gathers and scores them (fl_reads_push_bam) and pass 2 writes BAM. It always takes this path: its errors are
 //     thrown from here (nothing reaches stdout), and --verbose with it is one of them.
+//   * input that can be read only once (standard input, a pipe: streamsrc.h) is held in memory. Its plain text is cut
+//     into chunks as it arrives, and with one GPU each chunk is scored while the next is still arriving; gzip, BAM, or
+//     --gpus N > 1 read the stream to its end first and then go as a file does.
 // Anything else -- CR LF, multi-line records, broken records, a gzip file that is damaged or would not fit in memory,
 // --verbose -- makes run_text_feeder return handled == false before anything was printed to stdout, and main() runs
-// the kseq-compatible host parser.
+// the kseq-compatible host parser (over the stream's bytes in memory, once it has ended, for a stream).
 #pragma once
 #include <functional>
 
 #include "arguments.h"
 #include "kmers.h"
 
+class StreamInput;
+
 struct FeederOutcome {
     bool handled = false;      // false: nothing was done; use the host parser
     int exit_code = 0;
 };
 
-FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, const std::function<void(const char *)> &mark);
+// stream: the input reads when they are a stream (read already started), else nullptr
+FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, StreamInput *stream, const std::function<void(const char *)> &mark);

@@ -113,6 +113,8 @@ bool inflate_members(const unsigned char *d, const std::vector<Member> &ms, size
 
 }  // namespace
 
+uint64_t input_memory_budget() { return mem_available_bytes() / 10 * 6; }
+
 bool inflate_gzip_memory(const unsigned char *d, uint64_t n, InflatedInput &out, int max_threads, uint64_t budget, std::string *why) {
     auto fail = [&](const char *msg) {
         if (why) *why = msg;
@@ -121,7 +123,7 @@ bool inflate_gzip_memory(const unsigned char *d, uint64_t n, InflatedInput &out,
     };
     out.release();
     if (n < 18 || d[0] != 0x1f || d[1] != 0x8b) return fail("not a gzip file");
-    if (budget == 0) budget = mem_available_bytes() / 10 * 6;
+    if (budget == 0) budget = input_memory_budget();
     if (budget == 0) return fail("cannot tell how much memory is available");
 
     // ---- BGZF: sizes known, members independent ----

@@ -35,7 +35,10 @@ struct InflatedInput {
     }
 };
 
+// How much memory an input held in memory may take: 60 % of MemAvailable (0 when it cannot be told).
+uint64_t input_memory_budget();
+
 // `data`/`n`: the compressed file's bytes (e.g. a read-only mapping). max_threads <= 0: pick from the machine.
-// budget_bytes == 0: 60 % of MemAvailable.
+// budget_bytes == 0: input_memory_budget().
 bool inflate_gzip_memory(const unsigned char *data, uint64_t n, InflatedInput &out, int max_threads, uint64_t budget_bytes,
                          std::string *why);

@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <iostream>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <thread>
@@ -21,6 +22,7 @@
 #include "kmers.h"
 #include "misc.h"
 #include "read.h"
+#include "streamsrc.h"
 #include "survivors.h"
 #include "textsrc.h"
 
@@ -40,6 +42,9 @@ struct PhaseTimer {
         snprintf(buf, sizeof buf, "[timing] %-28s %8.3f s\n", what, std::chrono::duration<double>(now - last).count());
         report += buf;
         last = now;
+    }
+    void note(const char *what) {
+        if (on) report += std::string("[timing] ") + what + "\n";
     }
     ~PhaseTimer() {
         if (!on) return;
@@ -61,6 +66,10 @@ int main(int argc, char **argv) {
     std::ios::sync_with_stdio(false);
     std::cerr << "\n";
     PhaseTimer timer;
+    // Input that can be read only once (a pipe, standard input) is held in memory; reading it starts now, so that its
+    // producer is not blocked on a full pipe while the reference k-mers are built
+    StreamInput stream;
+    const bool streamed = stream_input(&args.input_reads);
     // The CUDA driver and context take about a second to come up: start that now, on
     // its own thread, and parse / pack the first records meanwhile (Kmers creates its context on
     // first use). Joined on every way out of main.
@@ -69,6 +78,7 @@ int main(int argc, char **argv) {
         ~Warmup() { if (t.joinable()) t.join(); }
     } warmup;
     try {
+        if (streamed) stream.start(args.input_reads);
         Kmers kmers;                                                      // main.cpp:53-59
         if (args.assembly_set) kmers.add_assembly_fasta(args.assembly);
         if (!args.short_reads.empty()) kmers.add_read_fastqs(args.short_reads);
@@ -77,9 +87,18 @@ int main(int argc, char **argv) {
 
         // ---- the device-first input path: the file as text to the device, survivors straight from the mapping ----
         {
-            const FeederOutcome fo = run_text_feeder(args, kmers, [&](const char *what) { timer.mark(what); });
+            const FeederOutcome fo = run_text_feeder(args, kmers, streamed ? &stream : nullptr, [&](const char *what) { timer.mark(what); });
+            if (streamed) {
+                char buf[160];
+                snprintf(buf, sizeof buf, "stream: %llu bytes, %zu of %zu chunks scored before its end",
+                         (unsigned long long)stream.stream_bytes(), stream.chunks_before_end.load(), stream.chunks.load());
+                timer.note(buf);
+            }
             if (fo.handled) return fo.exit_code;
         }
+        std::string why;
+        if (streamed && !stream.finish(&why)) throw std::runtime_error(why);
+        const MappedFile &mem = stream.file();                           // a stream: the whole input, in memory
 
         // ---- pass 1: parse, pack and score (main.cpp:61-130) ----
         long long total_bases = 0, last_progress = 0;
@@ -106,7 +125,8 @@ int main(int argc, char **argv) {
             }
         };
         {
-            FastxReader in(args.input_reads);
+            std::unique_ptr<FastxReader> reader(streamed ? new FastxReader(mem.base, mem.size) : new FastxReader(args.input_reads));
+            FastxReader &in = *reader;
             while (true) {
                 int64_t l64 = in.ok() ? in.next() : -1;
                 int l = (int)l64;                                         // main.cpp:69,77 (int truncation)
@@ -193,9 +213,11 @@ int main(int argc, char **argv) {
         const Format fmt{any_fasta ? '>' : '@', any_fastq};
         fl_ctx *bgzf = args.bgzip ? kmers.context() : nullptr;           // --bgzip: compressed on the scoring context's GPU
         MappedFile f;
-        const bool ok = table_ok && f.open_plain(args.input_reads) && table.within(f.size, fmt.quality)
-                            ? write_survivors(1, f.base, {Part{&table, Results::of(reads)}}, fmt, bgzf)
-                            : reparse_survivors(1, args.input_reads, Results::of(reads), reads.n_reads(), fmt, bgzf);
+        const MappedFile &src = streamed ? mem : f;
+        const bool ok = table_ok && (streamed || f.open_plain(args.input_reads)) && table.within(src.size, fmt.quality)
+                            ? write_survivors(1, src.base, {Part{&table, Results::of(reads)}}, fmt, bgzf)
+                        : streamed ? reparse_survivors(1, mem.base, mem.size, Results::of(reads), reads.n_reads(), fmt, bgzf)
+                                   : reparse_survivors(1, args.input_reads, Results::of(reads), reads.n_reads(), fmt, bgzf);
         timer.mark("pass 2 (parse, print)");
         std::cerr << "\n";
         if (!ok) return 1;

@@ -248,9 +248,10 @@ bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, c
     return write_survivors_writev(fd, base, parts, fmt);
 }
 
-bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+namespace {
+
+bool reparse(int fd, FastxReader &in, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
     fflush(stdout);
-    FastxReader in(path);
     auto run = [&](auto &sink) {
         for (size_t i = 0; in.ok() && in.next() >= 0 && i < n_reads; ++i) {
             const RecordText r{in.name.data(), in.name.size(), in.comment.data(), in.comment.size(), in.seq.data(), in.qual.data(),
@@ -268,6 +269,18 @@ bool reparse_survivors(int fd, const std::string &path, const Results &res, size
     run(c);
     c.flush();
     return !c.failed;
+}
+
+}  // namespace
+
+bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+    FastxReader in(path);
+    return reparse(fd, in, res, n_reads, fmt, bgzf);
+}
+
+bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+    FastxReader in(base, size);
+    return reparse(fd, in, res, n_reads, fmt, bgzf);
 }
 
 void log_after_trim_split(const Arguments &args, uint64_t n_rows, const fl_summary &summary) {

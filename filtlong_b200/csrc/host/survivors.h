@@ -79,6 +79,8 @@ bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &p
 bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);
 // Sequential: the survivors among the first n_reads records of `path`, parsed again.
 bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf);
+// The same over an input held in memory (a stream read once, streamsrc.h)
+bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf);
 
 // "  after trimming / splitting: N reads (B bp)" when --trim or --split is on, then a blank line (main.cpp:157-167)
 void log_after_trim_split(const Arguments &args, uint64_t n_rows, const fl_summary &summary);

@@ -88,29 +88,48 @@ bool record_starts_at(const char *b, uint64_t p, uint64_t size, int format) {
     return s3 <= size && e3 - s3 == e1 - s1;
 }
 
-}  // namespace
-
-bool plan_chunks(const char *b, uint64_t size, int format, uint64_t target, uint64_t max_chunk, std::vector<Chunk> &out) {
-    uint64_t pos = 0;
-    while (pos < size) {
-        uint64_t end = size;
-        if (size - pos > target) {
-            uint64_t p = pos + target;                         // last record start at or before pos + target
-            bool found = false;
-            while (p > pos) {
-                const void *q = memrchr(b + pos, '\n', (size_t)(p - pos));
-                if (!q) break;
-                const uint64_t cand = (uint64_t)((const char *)q - b) + 1;
-                if (cand > pos && record_starts_at(b, cand, size, format)) { end = cand; found = true; break; }
-                p = cand - 1;
-                if (pos + target - p > (64ull << 20)) break;    // a single record this large: give up on the fast path
-            }
-            if (!found) return false;
-        }
-        if (end - pos > max_chunk) return false;
-        out.push_back(Chunk{pos, end});
-        pos = end;
+// Have the four lines of a FASTQ record starting at p all arrived? Only then does record_starts_at over the bytes so far
+// answer what it answers over the whole input.
+bool lines_arrived(const char *b, uint64_t p, uint64_t avail, bool ended, int format) {
+    if (ended || format == FL_TEXT_FASTA) return true;
+    for (int i = 0; i < 4; ++i) {
+        const uint64_t e = eol(b, p, avail);
+        if (e >= avail) return false;
+        p = e + 1;
     }
     return true;
+}
+
+}  // namespace
+
+int plan_next_chunk(const char *b, uint64_t avail, bool ended, int format, uint64_t target, uint64_t max_chunk, uint64_t pos, Chunk *out) {
+    if (pos >= avail) return 0;
+    uint64_t end = avail;
+    if (avail - pos > target) {
+        uint64_t p = pos + target;                             // last record start at or before pos + target
+        bool found = false;
+        while (p > pos) {
+            const void *q = memrchr(b + pos, '\n', (size_t)(p - pos));
+            if (!q) break;
+            const uint64_t cand = (uint64_t)((const char *)q - b) + 1;
+            if (!lines_arrived(b, cand, avail, ended, format)) return 0;
+            if (cand > pos && record_starts_at(b, cand, avail, format)) { end = cand; found = true; break; }
+            p = cand - 1;
+            if (pos + target - p > (64ull << 20)) break;        // a single record this large: give up on the fast path
+        }
+        if (!found) return -1;
+    } else if (!ended) {
+        return 0;
+    }
+    if (end - pos > max_chunk) return -1;
+    *out = Chunk{pos, end};
+    return 1;
+}
+
+bool plan_chunks(const char *b, uint64_t size, int format, uint64_t target, uint64_t max_chunk, std::vector<Chunk> &out) {
+    Chunk c;
+    int r;
+    for (uint64_t pos = 0; (r = plan_next_chunk(b, size, true, format, target, max_chunk, pos, &c)) == 1; pos = c.end) out.push_back(c);
+    return r == 0;
 }
 

@@ -34,3 +34,9 @@ struct Chunk { uint64_t begin, end; };
 
 // record-aligned chunks of about `target` bytes; false if no boundary can be found (then the host parser runs)
 bool plan_chunks(const char *b, uint64_t size, int format, uint64_t target, uint64_t max_chunk, std::vector<Chunk> &out);
+
+// One step of plan_chunks over an input that is still arriving: the chunk that starts at `pos`, given the bytes [0, avail)
+// so far (`ended`: no more will come). 1: *out is that chunk; 0: wait for more bytes (or, once ended, nothing is left);
+// -1: no record start to cut at. A candidate cut is judged only once its record's four lines have arrived, so the chunks
+// cut while the input arrives are the ones plan_chunks cuts from the whole of it.
+int plan_next_chunk(const char *b, uint64_t avail, bool ended, int format, uint64_t target, uint64_t max_chunk, uint64_t pos, Chunk *out);
