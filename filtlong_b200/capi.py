@@ -107,6 +107,14 @@ class SynthReads(C.Structure):
 SYNTH_INDELS = 1
 
 
+class GunzipStats(C.Structure):
+    _fields_ = [("members", C.c_uint64), ("chunks", C.c_uint64), ("redecoded", C.c_uint64), ("rounds", C.c_uint64)]
+
+
+FL_GUNZIP_OK = 0
+FL_GUNZIP_DECLINED = 1
+
+
 # every symbol include/filtlong_b200.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = [
@@ -181,6 +189,10 @@ SYMBOLS = [
     ("fl_bgzf_bound", C.c_uint64, [C.c_uint64]),
     ("fl_bgzf_compress", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
     ("fl_bgzf_compress_device", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
+    ("fl_gzip_inflate", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64),
+                                  C.POINTER(C.c_int), C.POINTER(GunzipStats)]),
+    ("fl_gzip_inflate_device", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64),
+                                         C.POINTER(C.c_int), C.POINTER(GunzipStats)]),
     ("fl_version", C.c_char_p, []),
     ("fl_phred_luts", None, [C.c_int32, _P, _P]),
 ]

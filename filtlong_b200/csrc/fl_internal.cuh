@@ -233,6 +233,7 @@ struct fl_ctx {
     DevVec<unsigned long long> bz_offs;        // their output offsets
     DevVec<unsigned long long> bz_state;       // [0] bytes written so far, [1] the output buffer was too small
     DevVec<uint8_t> bz_hin, bz_hout;           // fl_bgzf_compress: the host buffers' device copies
+    bool inflate_attr_set = false;            // fl_gzip_inflate: k_inf_decode's shared memory limit is raised
     bool bgzf_attr_set = false;
 
     // ---- optional per-kernel timing (fl_ctx_enable_timing) ----

@@ -365,6 +365,11 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, StreamInput *stream
     FeederOutcome res;
     // per-read dumps come from the host path, which reads text only: a BAM input always takes this one
     const bool host_parser = args.verbose || getenv("FL_HOST_PARSER");
+    // FL_CLI_TIMING: the phase line, then which inflater ran (gzmem.h)
+    const auto mark_inflated = [&](const MappedFile &m) {
+        const std::string what = "gzip input inflated into memory (" + (m.inflater.empty() ? std::string("host threads") : m.inflater) + ")";
+        mark(what.c_str());
+    };
     MappedFile own;
     const MappedFile *fp = &own;
     std::string why;
@@ -377,9 +382,9 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, StreamInput *stream
         const char b0 = head ? stream->base()[0] : 0;
         growing = !host_parser && args.gpus == 1 && head >= 2 && (b0 == '@' || b0 == '>');
         if (growing) format = b0 == '@' ? FL_TEXT_FASTQ : FL_TEXT_FASTA;
-        else if (!stream->finish(&why)) throw std::runtime_error(why);
+        else if (!stream->finish(&why, kmers.device_inflater())) throw std::runtime_error(why);
         fp = &stream->file();
-        if (stream->inflated()) mark("gzip input inflated into memory");
+        if (stream->inflated()) mark_inflated(stream->file());
         if (!growing) {
             if (fp->size < 2 && !stream->inflated()) return res;        // as MappedFile::open_plain declines a file that small
             format = fp->format();
@@ -388,11 +393,11 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, StreamInput *stream
     } else {
         if (host_parser && !bam_file_magic(args.input_reads)) return res;
         bool inflated = false;
-        if (!own.open_any(args.input_reads, &inflated, &why)) {         // neither plain nor gzip that fits in memory: the host reader
+        if (!own.open_any(args.input_reads, &inflated, &why, kmers.device_inflater())) {   // neither plain nor gzip in memory: the host reader
             if (own.gzip && bam_file_magic(args.input_reads)) throw std::runtime_error("cannot read BAM input " + args.input_reads + ": " + why);
             return res;
         }
-        if (inflated) mark("gzip input inflated into memory");
+        if (inflated) mark_inflated(own);
         format = own.format();
     }
     const MappedFile &f = *fp;

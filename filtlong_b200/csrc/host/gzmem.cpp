@@ -115,7 +115,8 @@ bool inflate_members(const unsigned char *d, const std::vector<Member> &ms, size
 
 uint64_t input_memory_budget() { return mem_available_bytes() / 10 * 6; }
 
-bool inflate_gzip_memory(const unsigned char *d, uint64_t n, InflatedInput &out, int max_threads, uint64_t budget, std::string *why) {
+bool inflate_gzip_memory(const unsigned char *d, uint64_t n, InflatedInput &out, int max_threads, uint64_t budget, std::string *why,
+                         const GzipDeviceInflate &device) {
     auto fail = [&](const char *msg) {
         if (why) *why = msg;
         out.release();
@@ -180,6 +181,27 @@ bool inflate_gzip_memory(const unsigned char *d, uint64_t n, InflatedInput &out,
     out.reserved = page_round(want);
     out.base = reserve(out.reserved);
     if (!out.base) return fail("cannot reserve memory for the inflated input");
+    auto keep_used = [&](uint64_t used) {                              // give the unused tail of the reservation back
+        const uint64_t keep = page_round(used);
+        if (keep < out.reserved) {
+            munmap(out.base + keep, (size_t)(out.reserved - keep));
+            out.reserved = keep;
+        }
+    };
+    if (device) {
+        GzipDeviceResult r;
+        const bool ok = device(d, n, out.base, out.reserved, &r);
+        out.inflater = r.note;
+        if (ok && r.n_out) {
+            keep_used(r.n_out);
+            out.size = r.n_out;
+            out.members = (int)r.members;
+            out.threads = 0;
+            out.bgzf = false;
+            return true;
+        }
+        // declined: the host path below, on the same reservation (an empty result is the host's "empty input" too)
+    }
     z_stream zs;
     memset(&zs, 0, sizeof zs);
     if (inflateInit2(&zs, 15 + 16) != Z_OK) return fail("zlib: inflateInit2 failed");
@@ -213,12 +235,7 @@ bool inflate_gzip_memory(const unsigned char *d, uint64_t n, InflatedInput &out,
     inflateEnd(&zs);
     if (err) return fail(err);
     if (opos == 0) return fail("empty input");
-    // give the unused tail of the reservation back
-    const uint64_t keep = page_round(opos);
-    if (keep < out.reserved) {
-        munmap(out.base + keep, (size_t)(out.reserved - keep));
-        out.reserved = keep;
-    }
+    keep_used(opos);
     out.size = opos;
     out.members = members;
     out.threads = 1;

@@ -7,13 +7,15 @@
 //   * BGZF (bgzip: every member carries its compressed size in a 'BC' extra field and its inflated size in the
 //     trailer): the members are located without inflating anything, the output size is known up front, and the
 //     members are inflated in parallel by a few host threads, each straight into its final place;
-//   * any other gzip file (one member, or several concatenated): one thread, one z_stream, members back to back --
-//     what gzread does, including "bytes after the last member that do not start a gzip header are ignored".
+//   * any other gzip file (one member, or several concatenated): the caller's device inflater when it takes the file,
+//     else one thread, one z_stream, members back to back -- what gzread does, including "bytes after the last member
+//     that do not start a gzip header are ignored".
 // A file that is not gzip, is truncated or corrupt, or whose inflated size would not fit the memory budget (a share of
 // MemAvailable) yields `false` and leaves nothing behind: the caller then runs the kseq-compatible host reader, which
 // reports errors the way the reference does.
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <string>
 
 struct InflatedInput {
@@ -23,6 +25,7 @@ struct InflatedInput {
     int members = 0;             // gzip members inflated
     int threads = 1;             // host threads that inflated them
     bool bgzf = false;
+    std::string inflater;        // which inflater ran, for FL_CLI_TIMING: empty for the host threads
     InflatedInput() = default;
     InflatedInput(const InflatedInput &) = delete;
     InflatedInput &operator=(const InflatedInput &) = delete;
@@ -38,7 +41,17 @@ struct InflatedInput {
 // How much memory an input held in memory may take: 60 % of MemAvailable (0 when it cannot be told).
 uint64_t input_memory_budget();
 
+// An inflater tried before the host z_stream on a gzip file that is not BGZF (the CLI binds fl_gzip_inflate to its
+// scoring context). It writes out[0, cap) and returns true only when out[0, r->n_out) is exactly what zlib inflates from
+// data[0, n); false declines, and the host path then runs exactly as it would without it. r->note says what ran either
+// way (FL_CLI_TIMING). This file never calls into the CUDA library itself.
+struct GzipDeviceResult {
+    uint64_t n_out = 0, members = 0;
+    std::string note;
+};
+using GzipDeviceInflate = std::function<bool(const unsigned char *data, uint64_t n, char *out, uint64_t cap, GzipDeviceResult *r)>;
+
 // `data`/`n`: the compressed file's bytes (e.g. a read-only mapping). max_threads <= 0: pick from the machine.
-// budget_bytes == 0: input_memory_budget().
+// budget_bytes == 0: input_memory_budget(). device: see GzipDeviceInflate (empty: the host path only).
 bool inflate_gzip_memory(const unsigned char *data, uint64_t n, InflatedInput &out, int max_threads, uint64_t budget_bytes,
-                         std::string *why);
+                         std::string *why, const GzipDeviceInflate &device = GzipDeviceInflate());

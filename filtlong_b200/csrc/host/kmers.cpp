@@ -1,6 +1,7 @@
 // filtlong_b200/csrc/host/kmers.cpp -- see kmers.h. Log lines follow reference src/kmers.cpp:50-72.
 #include "kmers.h"
 
+#include <stdio.h>
 #include <stdlib.h>
 
 #include <iostream>
@@ -29,6 +30,45 @@ fl_ctx *Kmers::context() {
         if (rc != FL_OK) throw std::runtime_error(std::string("fl_ctx_create: ") + fl_last_error(nullptr));
     }
     return ctx_;
+}
+
+// The threshold is DESIGN §7's CLI sweep on an H100 (`filtlong -p 90` on one member of C2-like FASTQ at level 1, wall-clock,
+// best and median of 3 alternated runs): from 64 MiB compressed both favour the GPU inflater (256 MiB: 2.0 s against
+// 4.0 s); at 16 MiB and below the two are within the runs' spread, so the host z_stream keeps those files.
+// FL_GUNZIP_HOST=1 keeps every file on the host z_stream; FL_GUNZIP_MIN_BYTES=N moves the threshold (measurement only:
+// the bytes are the same either way).
+GzipDeviceInflate Kmers::device_inflater() {
+    return [this](const unsigned char *d, uint64_t n, char *out, uint64_t cap, GzipDeviceResult *r) {
+        uint64_t min_bytes = kDeviceGunzipMinBytes;
+        if (const char *e = getenv("FL_GUNZIP_MIN_BYTES")) min_bytes = strtoull(e, nullptr, 10);
+        if (n < min_bytes) { r->note = "host zlib (under the GPU inflater's threshold)"; return false; }
+        if (getenv("FL_GUNZIP_HOST")) { r->note = "host zlib (FL_GUNZIP_HOST)"; return false; }
+        fl_ctx *c = nullptr;
+        try {
+            c = context();
+        } catch (const std::exception &) {
+            r->note = "host zlib (no CUDA context)";
+            return false;
+        }
+        uint64_t got = 0;
+        int status = FL_GUNZIP_DECLINED;
+        fl_gunzip_stats st{};
+        const int rc = fl_gzip_inflate(c, d, n, out, cap, 0, 0, &got, &status, &st);
+        char buf[200];
+        if (rc != FL_OK) {
+            snprintf(buf, sizeof buf, "host zlib (GPU inflater failed: %.120s)", fl_last_error(c));
+            r->note = buf;
+            return false;
+        }
+        snprintf(buf, sizeof buf, "%s: %llu chunks, %llu re-decoded, %llu rounds",
+                 status == FL_GUNZIP_OK ? "GPU inflater" : "host zlib (GPU inflater declined)", (unsigned long long)st.chunks,
+                 (unsigned long long)st.redecoded, (unsigned long long)st.rounds);
+        r->note = buf;
+        if (status != FL_GUNZIP_OK) return false;
+        r->n_out = got;
+        r->members = st.members;
+        return true;
+    };
 }
 
 Kmers::~Kmers() {
@@ -101,7 +141,11 @@ int Kmers::add_reference(const std::string &filename, bool multi) {
     MappedFile f;
     std::vector<Chunk> plan;
     const bool timing = getenv("FL_CLI_TIMING") != nullptr;
-    bool text_path = !getenv("FL_HOST_PARSER") && f.open_any(filename) && (f.format() == FL_TEXT_FASTQ || f.format() == FL_TEXT_FASTA);
+    bool inflated = false;
+    bool text_path = !getenv("FL_HOST_PARSER") && f.open_any(filename, &inflated, nullptr, device_inflater()) &&
+                     (f.format() == FL_TEXT_FASTQ || f.format() == FL_TEXT_FASTA);
+    if (timing && inflated) std::cerr << "[timing] reference " << filename << ": gzip input inflated into memory, "
+                                      << (f.inflater.empty() ? std::string("host threads") : f.inflater) << "\n";
     if (text_path) {
         // a chunk holds whole records: FASTA chunks are large enough for a chromosome on one line or wrapped
         uint64_t target = f.format() == FL_TEXT_FASTA ? 512ull << 20 : 128ull << 20;

@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../../include/filtlong_b200.h"
+#include "gzmem.h"
 
 class Kmers {
 public:
@@ -31,6 +32,10 @@ public:
     // additions of the CUDA build
     uint64_t size();               // m_kmers.size()
     fl_ctx *context();
+    // fl_gzip_inflate on context(), for inflate_gzip_memory (gzmem.h): tried on gzip input that is not BGZF and has at
+    // least kDeviceGunzipMinBytes compressed bytes; a decline or a CUDA failure leaves the file to the host z_stream.
+    GzipDeviceInflate device_inflater();
+    static constexpr uint64_t kDeviceGunzipMinBytes = 64ull << 20;
     static void check(fl_ctx *ctx, int rc, const char *what);          // throws on a non-zero status
 
 private:

@@ -97,7 +97,7 @@ int main(int argc, char **argv) {
             if (fo.handled) return fo.exit_code;
         }
         std::string why;
-        if (streamed && !stream.finish(&why)) throw std::runtime_error(why);
+        if (streamed && !stream.finish(&why, kmers.device_inflater())) throw std::runtime_error(why);
         const MappedFile &mem = stream.file();                           // a stream: the whole input, in memory
 
         // ---- pass 1: parse, pack and score (main.cpp:61-130) ----

@@ -126,7 +126,7 @@ uint64_t StreamInput::stream_bytes() {
     return got_;
 }
 
-bool StreamInput::finish(std::string *why) {
+bool StreamInput::finish(std::string *why, const GzipDeviceInflate &device) {
     if (!finished_) {
         finished_ = true;
         if (reader_.joinable()) reader_.join();
@@ -143,12 +143,13 @@ bool StreamInput::finish(std::string *why) {
             std::string iw;
             if (n >= budget_) {
                 w = name_ + " did not fit in memory once inflated";
-            } else if (inflate_gzip_memory((const unsigned char *)buf_, n, in, threads, budget_ - n, &iw)) {
+            } else if (inflate_gzip_memory((const unsigned char *)buf_, n, in, threads, budget_ - n, &iw, device)) {
                 munmap(buf_, (size_t)file_.map_bytes);                // the compressed bytes are not needed any more
                 buf_ = nullptr;
                 file_.size = in.size;
                 file_.map_bytes = in.reserved;
                 file_.base = in.take();
+                file_.inflater = in.inflater;
                 inflated_ = true;
                 finish_ok_ = true;
             } else if (iw == "empty input") {                          // like an empty file

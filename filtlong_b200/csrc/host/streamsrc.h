@@ -38,7 +38,7 @@ public:
     const char *base() const { return file_.base; }
     // Waits for the end of the stream and inflates a gzip stream. false: *why says what went wrong (the stream did not fit
     // in memory, could not be read, or is a damaged gzip stream). Then file() is the whole input, in memory (fd < 0).
-    bool finish(std::string *why);
+    bool finish(std::string *why, const GzipDeviceInflate &device = GzipDeviceInflate());
     const MappedFile &file() const { return file_; }
     bool inflated() const { return inflated_; }
     uint64_t stream_bytes();                                    // bytes read from the stream so far (compressed, for gzip)

@@ -26,12 +26,14 @@ bool MappedFile::open_plain(const std::string &path) {
     return !gzip;
 }
 
-bool MappedFile::inflate(std::string *why) {
+bool MappedFile::inflate(std::string *why, const GzipDeviceInflate &device) {
     if (!gzip || !base) return false;
     InflatedInput in;
     int threads = 0;
     if (const char *e = getenv("FL_INFLATE_THREADS")) threads = atoi(e);
-    if (!inflate_gzip_memory((const unsigned char *)base, size, in, threads, 0, why)) return false;
+    const bool ok = inflate_gzip_memory((const unsigned char *)base, size, in, threads, 0, why, device);
+    inflater = in.inflater;
+    if (!ok) return false;
     munmap((void *)base, (size_t)map_bytes);
     ::close(fd);
     fd = -1;
@@ -41,14 +43,14 @@ bool MappedFile::inflate(std::string *why) {
     return true;
 }
 
-bool MappedFile::open_any(const std::string &path, bool *inflated, std::string *why) {
+bool MappedFile::open_any(const std::string &path, bool *inflated, std::string *why, const GzipDeviceInflate &device) {
     if (inflated) *inflated = false;
     if (open_plain(path)) return true;
     std::string w;
     if (!why) why = &w;
     if (!gzip) return false;                                           // not gzip either
     if (getenv("FL_GZ_HOST")) { *why = "FL_GZ_HOST is set"; return false; }
-    if (!inflate(why)) return false;                                   // declined (gzmem.h)
+    if (!inflate(why, device)) return false;                           // declined (gzmem.h)
     if (inflated) *inflated = true;
     return true;
 }

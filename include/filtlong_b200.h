@@ -397,6 +397,34 @@ int fl_bgzf_compress(fl_ctx *ctx, const void *host_in, uint64_t n, void *host_ou
 int fl_bgzf_compress_device(fl_ctx *ctx, const void *dev_in, uint64_t n, void *dev_out, uint64_t cap, int append_eof,
                             uint64_t *n_out);
 
+/* ---- gzip input inflated on the device (no reference counterpart: the reference reads .gz input through zlib's gzread)
+ * An ordinary gzip file -- one member, or several back to back, with whatever bytes after the last member that do not
+ * start a gzip header, as gzread reads it -- inflated in parallel on the context's device: chunks of the compressed
+ * bytes are decoded speculatively from candidate block starts, the chain of chunk boundaries is checked and repaired,
+ * back-references into a chunk's unknown 32 KiB window are resolved afterwards, and every member's CRC-32 and ISIZE are
+ * checked. Output symbols take 2 bytes per output byte on the device, so a large file is done in rounds sized from the
+ * free device memory. bin/filtlong uses it on its scoring context for gzip input that is not BGZF and has at least
+ * 64 MiB of compressed bytes, and falls back to one host zlib thread on a decline.
+ * FL_GUNZIP_OK: host_out[0, *n_out) holds exactly the bytes zlib inflates from host_in. FL_GUNZIP_DECLINED: anything
+ * not handled here -- not gzip, truncated, corrupt, a bad CRC or ISIZE, more than cap bytes, a chunk whose output does
+ * not fit its slot, too many repair passes, not enough device memory -- and nothing is promised about host_out.
+ * chunk_bytes / max_device_bytes: 0 = the library's choice (max_device_bytes is then the free device memory).
+ * Works on any context and leaves its reads and results as they are; every device buffer is freed before it returns.
+ * A CUDA failure is FL_ECUDA. */
+enum { FL_GUNZIP_OK = 0, FL_GUNZIP_DECLINED = 1 };
+typedef struct fl_gunzip_stats {
+    uint64_t members;      /* gzip members inflated */
+    uint64_t chunks;       /* chunks decoded (a chunk without a candidate start is merged into the one before) */
+    uint64_t redecoded;    /* chunks decoded again from where their predecessor really stopped */
+    uint64_t rounds;       /* rounds of chunks the device memory allowed */
+} fl_gunzip_stats;
+/* Host buffers (the CLI's path: a mapped file into the reservation it is read from). */
+int fl_gzip_inflate(fl_ctx *ctx, const void *host_in, uint64_t n, void *host_out, uint64_t cap, uint64_t chunk_bytes,
+                    uint64_t max_device_bytes, uint64_t *n_out, int *status, fl_gunzip_stats *stats);
+/* Device buffers on the context's device: the same, without the copies. */
+int fl_gzip_inflate_device(fl_ctx *ctx, const void *dev_in, uint64_t n, void *dev_out, uint64_t cap, uint64_t chunk_bytes,
+                           uint64_t max_device_bytes, uint64_t *n_out, int *status, fl_gunzip_stats *stats);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char *fl_version(void);
 /* Phred look-up tables exactly as the device uses them (read.cpp:270-273 evaluated with the host
