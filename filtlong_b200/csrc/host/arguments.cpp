@@ -10,6 +10,7 @@
 #include <sstream>
 #include <stdexcept>
 
+#include <fcntl.h>
 #include <sys/stat.h>
 #include <unistd.h>
 
@@ -104,6 +105,7 @@ const Opt kOpts[] = {
     {0, "window_size", true, "int", "size of sliding window used when measuring window quality (default: 250)"},
     {0, "gpus", true, "int", "number of GPUs to shard the read set across (default: 1; not a reference option)"},
     {0, "bgzip", false, "bgzip", "compress the output as BGZF (gzip-compatible) on the GPU (not a reference option)"},
+    {0, "failed", true, "file", "write the reads that are not kept to this file (not a reference option)"},
     {0, "verbose", false, "verbose", "verbose output to stderr with info for each read"},
     {0, "version", false, "version", "display the program version and quit"},
     {'h', "help", false, "help", "display this help menu"},
@@ -120,7 +122,7 @@ void print_help(const char *prog) {
         {"external references (if provided, read quality will be determined using these instead of from the Phred scores):", 6, 8},
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
         {"read manipulation:", 12, 13},
-        {"other:", 14, 19},
+        {"other:", 14, 20},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -165,6 +167,7 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "window_size") window_ll = read_plain_ll(nm, v);
         else if (ln == "gpus") gpus = (int)read_plain_ll(nm, v);
         else if (ln == "bgzip") bgzip = true;
+        else if (ln == "failed") { failed = v; failed_set = true; }
         else if (ln == "verbose") verbose = true;
         else if (ln == "version") version_flag = true;
         else if (ln == "help") throw HelpRequested();
@@ -255,6 +258,22 @@ Arguments::Arguments(int argc, char **argv) {
     if (split_set && split <= 0) FAIL("Error: the value for --split must be a positive integer");
     if (window_size <= 0) FAIL("Error: the value for --window_size must be a positive integer");
     if (gpus < 1 || gpus > 64) FAIL("Error: the value for --gpus must be between 1 and 64");
+    if (failed_set) {
+        // checked, then opened (and truncated), before any read is scored
+        if (failed == "-") FAIL("Error: --failed needs a file: standard output carries the kept reads");
+        struct stat fs, st;
+        if (stat(failed.c_str(), &fs) == 0) {
+            auto same = [&](const struct stat &o) { return o.st_dev == fs.st_dev && o.st_ino == fs.st_ino; };
+            std::vector<std::string> inputs = files;
+            if (input_reads != "-") inputs.push_back(input_reads);
+            for (const auto &in : inputs)
+                if (stat(in.c_str(), &st) == 0 && same(st)) FAIL("Error: --failed must not be an input file: " + failed);
+            if (input_reads == "-" && fstat(0, &st) == 0 && same(st)) FAIL("Error: --failed must not be an input file: " + failed);
+            if (fstat(1, &st) == 0 && same(st)) FAIL("Error: --failed must not be standard output: " + failed);
+        }
+        failed_fd = open(failed.c_str(), O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0666);
+        if (failed_fd < 0) FAIL("Error: cannot write to file: " + failed);
+    }
 }
 
 bool Arguments::does_file_exist(const std::string &filename) {

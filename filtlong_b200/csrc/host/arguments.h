@@ -44,6 +44,10 @@ public:
     bool verbose = false;
     int gpus = 1;                 // this build only: shard the read set across this many GPUs (one context + one thread each)
     bool bgzip = false;           // this build only: stdout compressed as BGZF on the GPU (bgzf_out.h)
+    // this build only: the rows stdout does not get go to this file, opened (O_TRUNC) while the arguments are checked
+    bool failed_set = false;
+    std::string failed;
+    int failed_fd = -1;
 
 private:
     bool does_file_exist(const std::string &filename);

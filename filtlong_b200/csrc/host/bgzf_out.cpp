@@ -12,6 +12,10 @@ namespace {
 // the empty member that ends a BGZF file (SAM specification 4.1.2)
 const unsigned char kEof[28] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 'B', 'C', 2, 0, 0x1b, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
+// held around every fl_bgzf_compress call of every BgzfOut: a context takes one host thread at a time, and the re-parse
+// path of pass 2 runs two BgzfOut (stdout and --failed) on one context
+std::mutex g_compress;
+
 bool write_all(int fd, const char *p, uint64_t n) {
     while (n) {
         const ssize_t w = write(fd, p, (size_t)n);
@@ -94,10 +98,15 @@ void BgzfOut::compress_loop() {
             std::lock_guard<std::mutex> lk(m_);
             ok = !failed_;
         }
-        if (ok && fl_bgzf_compress(ctx_, in_[i], in_len_[i], out_[o], out_cap_, 0, &n) != FL_OK) {
-            std::lock_guard<std::mutex> lk(m_);
-            fail(std::string("fl_bgzf_compress: ") + fl_last_error(ctx_));
-            ok = false;
+        if (ok) {
+            std::unique_lock<std::mutex> gl(g_compress);
+            if (fl_bgzf_compress(ctx_, in_[i], in_len_[i], out_[o], out_cap_, 0, &n) != FL_OK) {
+                const std::string why = std::string("fl_bgzf_compress: ") + fl_last_error(ctx_);
+                gl.unlock();
+                std::lock_guard<std::mutex> lk(m_);
+                fail(why);
+                ok = false;
+            }
         }
         std::lock_guard<std::mutex> lk(m_);
         in_busy_[i] = false;

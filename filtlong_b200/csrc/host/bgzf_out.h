@@ -5,7 +5,9 @@
 // blocks, each batch is compressed by fl_bgzf_compress and the members are written to the descriptor in order. Filling
 // the next batch (the caller's thread), compressing one (a compressor thread) and writing the one before (a writer
 // thread) overlap. finish() writes the last batch and the EOF member. The context must not be used by anyone else
-// until finish() returns.
+// until finish() returns, except by other BgzfOut: all of them in the process share one lock around fl_bgzf_compress, so
+// two sinks on one context (stdout and `--failed` in one re-parse) compress one batch at a time, in turn, on the same
+// GPU, while their fills and writes still overlap.
 #pragma once
 #include <condition_variable>
 #include <cstddef>

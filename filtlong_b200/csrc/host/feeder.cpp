@@ -566,7 +566,10 @@ FeederOutcome run_text_feeder(Arguments &args, Kmers &kmers, StreamInput *stream
     for (auto &s : shards) parts.push_back(Part{&s.rec, Results::of(s)});
     const Format fmt{format == FL_TEXT_FASTA ? '>' : '@', format == FL_TEXT_FASTQ, bam, bam_header_bytes};
     // BAM in, BAM out: always BGZF (--bgzip changes nothing)
-    const bool out_failed = !write_survivors(g_out_fd, f.base, parts, fmt, args.bgzip || bam ? ctx0 : nullptr);
+    fl_ctx *bgzf = args.bgzip || bam ? ctx0 : nullptr;
+    bool out_failed = !write_survivors(g_out_fd, f.base, parts, fmt, bgzf);
+    // --failed: the other rows, a second walk over the same table
+    if (args.failed_fd >= 0 && !report_failed_write(args, write_survivors(args.failed_fd, f.base, parts, fmt, bgzf, false))) out_failed = true;
     mark("pass 2 (slices of the mapped input)");
     std::cerr << "\n";
     cleanup();

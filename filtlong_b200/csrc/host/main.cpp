@@ -214,10 +214,19 @@ int main(int argc, char **argv) {
         fl_ctx *bgzf = args.bgzip ? kmers.context() : nullptr;           // --bgzip: compressed on the scoring context's GPU
         MappedFile f;
         const MappedFile &src = streamed ? mem : f;
-        const bool ok = table_ok && (streamed || f.open_plain(args.input_reads)) && table.within(src.size, fmt.quality)
-                            ? write_survivors(1, src.base, {Part{&table, Results::of(reads)}}, fmt, bgzf)
-                        : streamed ? reparse_survivors(1, mem.base, mem.size, Results::of(reads), reads.n_reads(), fmt, bgzf)
-                                   : reparse_survivors(1, args.input_reads, Results::of(reads), reads.n_reads(), fmt, bgzf);
+        // --failed: the other rows to args.failed_fd, by a second walk over the table or in the same re-parse
+        const int failed_fd = args.failed_fd;
+        bool ok, failed_ok = true;
+        if (table_ok && (streamed || f.open_plain(args.input_reads)) && table.within(src.size, fmt.quality)) {
+            const std::vector<Part> parts{Part{&table, Results::of(reads)}};
+            ok = write_survivors(1, src.base, parts, fmt, bgzf);
+            if (failed_fd >= 0) failed_ok = write_survivors(failed_fd, src.base, parts, fmt, bgzf, false);
+        } else if (streamed) {
+            ok = reparse_survivors(1, mem.base, mem.size, Results::of(reads), reads.n_reads(), fmt, bgzf, failed_fd, &failed_ok);
+        } else {
+            ok = reparse_survivors(1, args.input_reads, Results::of(reads), reads.n_reads(), fmt, bgzf, failed_fd, &failed_ok);
+        }
+        if (failed_fd >= 0 && !report_failed_write(args, failed_ok)) ok = false;
         timer.mark("pass 2 (parse, print)");
         std::cerr << "\n";
         if (!ok) return 1;

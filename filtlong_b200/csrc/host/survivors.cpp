@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstring>
 #include <iostream>
+#include <memory>
 #include <thread>
 
 #include "bam.h"
@@ -55,20 +56,22 @@ RecordText text_of(const Records &R, const char *base, size_t i) {
 // end the reference's substr throws; here nothing is printed (DESIGN 5).
 size_t c_substr(size_t n, size_t start, size_t length) { return start >= n ? 0 : std::min(length, n - start); }
 
-// Read i's output: the read if it survived and has no children, else each surviving child longer than 0. put()'s bytes
-// must stay valid until the sink is flushed; put_owned() keeps its string alive until then.
+// Read i's output: the read if its pass flag is `want` and it has no children, else each child longer than 0 whose flag
+// is `want` (stdout: the survivors, want = true; --failed: the rest, want = false). put()'s bytes must stay valid until
+// the sink is flushed; put_owned() keeps its string alive until then.
 template <class Sink>
-void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Results &res, size_t i) {
+void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Results &res, size_t i, bool want) {
+    auto pass = [&](size_t row) { return (res.row_pfinal[row] != 0) == want; };
     if (fmt.bam) {                                                        // the record as it is, or new ones for the children
         const char *rec = bam_record_of(r.name);
         const size_t rs = (size_t)res.row_start[i];
         if (res.n_child[i] == 0) {
-            if (res.row_pfinal[rs]) sink.put(rec, bam_record_bytes(rec));
+            if (pass(rs)) sink.put(rec, bam_record_bytes(rec));
             return;
         }
         for (size_t row = rs; row < rs + (size_t)res.n_child[i]; ++row) {
             const int start = res.row_s[row], end = res.row_e[row];
-            if (!res.row_pfinal[row] || end - start <= 0 || (size_t)end > r.len) continue;
+            if (!pass(row) || end - start <= 0 || (size_t)end > r.len) continue;
             std::string child;
             bam_child_record(rec, start, end, child);
             sink.put_owned(std::move(child));
@@ -85,7 +88,7 @@ void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Re
     };
     const size_t rs = (size_t)res.row_start[i];
     if (res.n_child[i] == 0) {
-        if (!res.row_pfinal[rs]) return;
+        if (!pass(rs)) return;
         if (r.lead_before_name) sink.put(r.name - 1, 1 + r.name_len);
         else { sink.put(lead, 1); sink.put(r.name, r.name_len); }
         rest(0, r.len);
@@ -94,7 +97,7 @@ void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Re
     for (size_t row = rs; row < rs + (size_t)res.n_child[i]; ++row) {
         const int start = res.row_s[row], end = res.row_e[row];
         // (a row past the record's end can only come from an input that changed since pass 1)
-        if (!res.row_pfinal[row] || end - start <= 0 || (size_t)end > r.len) continue;
+        if (!pass(row) || end - start <= 0 || (size_t)end > r.len) continue;
         std::string nm(lead, 1);
         append_child_name(nm, r.name, r.name_len, start, end);
         sink.put_owned(std::move(nm));
@@ -103,8 +106,8 @@ void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Re
 }
 
 template <class Sink>
-void emit_range(Sink &sink, const char *base, const Part &p, size_t lo, size_t hi, const Format &fmt) {
-    for (size_t i = lo; i < hi; ++i) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i);
+void emit_range(Sink &sink, const char *base, const Part &p, size_t lo, size_t hi, const Format &fmt, bool want) {
+    for (size_t i = lo; i < hi; ++i) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i, want);
 }
 
 // iovecs into the mapping, written with writev()
@@ -177,15 +180,15 @@ bool finish(BgzfOut &z) {
 
 }  // namespace
 
-bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt) {
+bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want) {
     Writer w(fd);
-    for (const Part &p : parts) emit_range(w, base, p, 0, p.rec->n, fmt);
+    for (const Part &p : parts) emit_range(w, base, p, 0, p.rec->n, fmt, want);
     w.flush();
     return !w.failed;
 }
 
 // contiguous groups of reads are sized, then written with pwrite() by a few threads
-bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt) {
+bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want) {
     struct Group { size_t part, lo, hi; uint64_t bytes = 0, at = 0; };
     std::vector<Group> groups;
     size_t n_reads = 0;
@@ -205,11 +208,11 @@ bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &p
                     Group &G = groups[g];
                     if (!write_pass) {
                         Sizer z;
-                        emit_range(z, base, parts[G.part], G.lo, G.hi, fmt);
+                        emit_range(z, base, parts[G.part], G.lo, G.hi, fmt, want);
                         G.bytes = z.n;
                     } else {
                         Copier c(fd, (int64_t)base_pos + (int64_t)G.at);
-                        emit_range(c, base, parts[G.part], G.lo, G.hi, fmt);
+                        emit_range(c, base, parts[G.part], G.lo, G.hi, fmt, want);
                         c.flush();
                         if (c.failed) bad.store(true);
                     }
@@ -225,62 +228,79 @@ bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &p
     return lseek(fd, base_pos + (off_t)total_out, SEEK_SET) >= 0;
 }
 
-bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf) {
+bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want) {
     fflush(stdout);
     if (bgzf) {
         // compressed offsets are not known in advance: pipe or file, the members are written in order
         BgzfOut z(bgzf, fd);
         if (fmt.bam) z.put(base, (size_t)fmt.bam_header);
-        for (const Part &p : parts) emit_range(z, base, p, 0, p.rec->n, fmt);
+        for (const Part &p : parts) emit_range(z, base, p, 0, p.rec->n, fmt, want);
         return finish(z);
     }
     if (fmt.bam) {
         Copier c(fd, -1);
         c.put(base, (size_t)fmt.bam_header);
-        for (const Part &p : parts) emit_range(c, base, p, 0, p.rec->n, fmt);
+        for (const Part &p : parts) emit_range(c, base, p, 0, p.rec->n, fmt, want);
         c.flush();
         return !c.failed;
     }
     struct stat st;
     const int flags = fcntl(fd, F_GETFL);
     if (fstat(fd, &st) == 0 && S_ISREG(st.st_mode) && flags >= 0 && !(flags & O_APPEND))
-        return write_survivors_pwrite(fd, base, parts, fmt);
-    return write_survivors_writev(fd, base, parts, fmt);
+        return write_survivors_pwrite(fd, base, parts, fmt, want);
+    return write_survivors_writev(fd, base, parts, fmt, want);
 }
 
 namespace {
 
-bool reparse(int fd, FastxReader &in, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+// One walk over the input feeds both outputs: stdout's sink, and failed's when there is one (a null pointer otherwise)
+bool reparse(int fd, FastxReader &in, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf, int failed_fd, bool *failed_ok) {
     fflush(stdout);
-    auto run = [&](auto &sink) {
+    auto run = [&](auto &sink, auto *failed) {
         for (size_t i = 0; in.ok() && in.next() >= 0 && i < n_reads; ++i) {
             const RecordText r{in.name.data(), in.name.size(), in.comment.data(), in.comment.size(), in.seq.data(), in.qual.data(),
                                in.seq.size(), false, !in.comment.empty(), strnlen(in.comment.data(), in.comment.size()),
                                strnlen(in.seq.data(), in.seq.size()), strnlen(in.qual.data(), in.qual.size())};
-            emit_survivors(sink, fmt, r, res, i);
+            emit_survivors(sink, fmt, r, res, i, true);
+            if (failed) emit_survivors(*failed, fmt, r, res, i, false);
         }
     };
-    if (bgzf) {
+    bool ok, second_ok = true;
+    if (bgzf) {                                   // two BgzfOut on one context: bgzf_out.h serialises their compressions
         BgzfOut z(bgzf, fd);
-        run(z);
-        return finish(z);
+        std::unique_ptr<BgzfOut> zf(failed_fd >= 0 ? new BgzfOut(bgzf, failed_fd) : nullptr);
+        run(z, zf.get());
+        ok = finish(z);
+        if (zf) second_ok = finish(*zf);
+    } else {
+        Copier c(fd, -1);
+        std::unique_ptr<Copier> cf(failed_fd >= 0 ? new Copier(failed_fd, -1) : nullptr);
+        run(c, cf.get());
+        c.flush();
+        ok = !c.failed;
+        if (cf) { cf->flush(); second_ok = !cf->failed; }
     }
-    Copier c(fd, -1);
-    run(c);
-    c.flush();
-    return !c.failed;
+    if (failed_ok) *failed_ok = second_ok;
+    return ok;
 }
 
 }  // namespace
 
-bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf, int failed_fd,
+                       bool *failed_ok) {
     FastxReader in(path);
-    return reparse(fd, in, res, n_reads, fmt, bgzf);
+    return reparse(fd, in, res, n_reads, fmt, bgzf, failed_fd, failed_ok);
 }
 
-bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf) {
+bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
+                       int failed_fd, bool *failed_ok) {
     FastxReader in(base, size);
-    return reparse(fd, in, res, n_reads, fmt, bgzf);
+    return reparse(fd, in, res, n_reads, fmt, bgzf, failed_fd, failed_ok);
+}
+
+bool report_failed_write(const Arguments &args, bool ok) {
+    if (!ok) std::cerr << "Error: cannot write to file: " << args.failed << "\n";
+    return ok;
 }
 
 void log_after_trim_split(const Arguments &args, uint64_t n_rows, const fl_summary &summary) {

@@ -6,7 +6,9 @@
 //     descriptor is a regular file not opened with O_APPEND; else to writev().
 //   * sequential: the input parsed again by FastxReader (streamed gzip, CR LF, multi-line records), copied through a
 //     buffer or into BGZF.
-// Every writer returns false when a write (or a compression) failed.
+// Every writer writes the rows whose final pass flag equals `want`: stdout gets the survivors (true), `--failed FILE` the
+// rest (false), with the same bytes a survivor would have. Every writer returns false when a write (or a compression)
+// failed.
 #pragma once
 #include <cstdint>
 #include <string>
@@ -73,14 +75,20 @@ inline void append_child_name(std::string &out, const char *name, size_t name_le
 // Random access: the survivors of `parts`, in order, from the input mapped at `base`; compressed on the context `bgzf`
 // when it is given. The last two are the choices write_survivors makes, callable directly. BAM (fmt.bam): the header,
 // then each kept read's record as it is and a new record for each kept child; the CLI always passes a context, without
-// one the uncompressed BAM stream is written.
-bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf);
-bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);
-bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt);
-// Sequential: the survivors among the first n_reads records of `path`, parsed again.
-bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf);
+// one the uncompressed BAM stream is written. A second output is a second call, on its descriptor with want = false.
+bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want = true);
+bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want = true);
+bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want = true);
+// Sequential: the survivors among the first n_reads records of `path`, parsed again. With failed_fd >= 0 the same parse
+// also writes the other rows to failed_fd (compressed too when bgzf is given), and *failed_ok (when given) tells whether
+// that output was written; the return value is stdout's.
+bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
+                       int failed_fd = -1, bool *failed_ok = nullptr);
 // The same over an input held in memory (a stream read once, streamsrc.h)
-bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf);
+bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
+                       int failed_fd = -1, bool *failed_ok = nullptr);
+// --failed: `ok`, after printing an error that names the file when it is false
+bool report_failed_write(const Arguments &args, bool ok);
 
 // "  after trimming / splitting: N reads (B bp)" when --trim or --split is on, then a blank line (main.cpp:157-167)
 void log_after_trim_split(const Arguments &args, uint64_t n_rows, const fl_summary &summary);
