@@ -18,6 +18,7 @@
 #include <zlib.h>
 
 #include <cstdint>
+#include <memory>
 #include <string>
 
 class FastxReader {
@@ -60,4 +61,20 @@ private:
     uint64_t pos() const { return buf_base_ + (uint64_t)begin_; }
     bool eof_ = false, err_ = false;
     int last_char_ = 0;
+};
+
+// Where a FastxReader reads its records from: a file by its path (plain or gzip, streamed through zlib), or bytes already
+// in memory. A path converts to one, so a caller that has only a path passes it as it is.
+struct FastxInput {
+    std::string path;
+    const char *mem = nullptr;
+    uint64_t n_bytes = 0;
+    bool in_memory = false;
+    FastxInput(const std::string &p) : path(p) {}
+    FastxInput(const char *p) : path(p) {}
+    FastxInput(const char *m, uint64_t n) : mem(m), n_bytes(n), in_memory(true) {}
+    // a reader at the first record
+    std::unique_ptr<FastxReader> open() const {
+        return std::unique_ptr<FastxReader>(in_memory ? new FastxReader(mem, n_bytes) : new FastxReader(path));
+    }
 };

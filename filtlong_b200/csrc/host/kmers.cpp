@@ -144,14 +144,10 @@ int Kmers::add_reference(const std::string &filename, bool multi) {
     bool inflated = false;
     bool text_path = !getenv("FL_HOST_PARSER") && f.open_any(filename, &inflated, nullptr, device_inflater()) &&
                      (f.format() == FL_TEXT_FASTQ || f.format() == FL_TEXT_FASTA);
-    if (timing && inflated) std::cerr << "[timing] reference " << filename << ": gzip input inflated into memory, "
-                                      << (f.inflater.empty() ? std::string("host threads") : f.inflater) << "\n";
+    if (timing && inflated) std::cerr << "[timing] reference " << filename << ": gzip input inflated into memory, " << f.inflater << "\n";
     if (text_path) {
         // a chunk holds whole records: FASTA chunks are large enough for a chromosome on one line or wrapped
-        uint64_t target = f.format() == FL_TEXT_FASTA ? 512ull << 20 : 128ull << 20;
-        if (const char *e = getenv("FL_CHUNK_MB")) target = (uint64_t)atoll(e) << 20;
-        if (target < (1ull << 20)) target = 1ull << 20;
-        if (target > (1024ull << 20)) target = 1024ull << 20;
+        const uint64_t target = chunk_target(f.format() == FL_TEXT_FASTA ? 512ull << 20 : 128ull << 20);
         text_path = plan_chunks(f.base, f.size, f.format(), target, target, plan) && !plan.empty();
     }
     if (text_path) {

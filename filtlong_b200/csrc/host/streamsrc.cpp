@@ -4,7 +4,6 @@
 #include <errno.h>
 #include <fcntl.h>
 #include <poll.h>
-#include <stdlib.h>
 #include <string.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
@@ -130,26 +129,19 @@ bool StreamInput::finish(std::string *why, const GzipDeviceInflate &device) {
     if (!finished_) {
         finished_ = true;
         if (reader_.joinable()) reader_.join();
-        const uint64_t n = got_;
+        const uint64_t n = file_.size = got_;
+        file_.gzip = n >= 2 && (unsigned char)buf_[0] == 0x1f && (unsigned char)buf_[1] == 0x8b;
         std::string &w = finish_why_;
         if (overflow_) {
             w = name_ + " did not fit in memory (more than " + std::to_string(budget_) + " bytes; the limit is 60 % of MemAvailable)";
         } else if (errno_) {
             w = "cannot read " + name_ + ": " + strerror(errno_);
-        } else if (n >= 2 && (unsigned char)buf_[0] == 0x1f && (unsigned char)buf_[1] == 0x8b) {
-            InflatedInput in;
-            int threads = 0;
-            if (const char *e = getenv("FL_INFLATE_THREADS")) threads = atoi(e);
+        } else if (file_.gzip) {
             std::string iw;
             if (n >= budget_) {
                 w = name_ + " did not fit in memory once inflated";
-            } else if (inflate_gzip_memory((const unsigned char *)buf_, n, in, threads, budget_ - n, &iw, device)) {
-                munmap(buf_, (size_t)file_.map_bytes);                // the compressed bytes are not needed any more
-                buf_ = nullptr;
-                file_.size = in.size;
-                file_.map_bytes = in.reserved;
-                file_.base = in.take();
-                file_.inflater = in.inflater;
+            } else if (file_.inflate(budget_ - n, &iw, device)) {
+                buf_ = nullptr;                                        // file_ gave the compressed bytes back
                 inflated_ = true;
                 finish_ok_ = true;
             } else if (iw == "empty input") {                          // like an empty file
@@ -159,7 +151,6 @@ bool StreamInput::finish(std::string *why, const GzipDeviceInflate &device) {
                 w = name_ + ": " + iw;
             }
         } else {
-            file_.size = n;
             finish_ok_ = true;
         }
     }

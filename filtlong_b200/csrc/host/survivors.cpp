@@ -251,10 +251,17 @@ bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, c
     return write_survivors_writev(fd, base, parts, fmt, want);
 }
 
-namespace {
+bool write_outputs(const Arguments &args, int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf) {
+    bool ok = write_survivors(fd, base, parts, fmt, bgzf);
+    if (args.failed_fd >= 0 && !report_failed_write(args, write_survivors(args.failed_fd, base, parts, fmt, bgzf, false))) ok = false;
+    return ok;
+}
 
 // One walk over the input feeds both outputs: stdout's sink, and failed's when there is one (a null pointer otherwise)
-bool reparse(int fd, FastxReader &in, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf, int failed_fd, bool *failed_ok) {
+bool reparse_survivors(int fd, const FastxInput &input, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
+                       int failed_fd, bool *failed_ok) {
+    const std::unique_ptr<FastxReader> reader = input.open();
+    FastxReader &in = *reader;
     fflush(stdout);
     auto run = [&](auto &sink, auto *failed) {
         for (size_t i = 0; in.ok() && in.next() >= 0 && i < n_reads; ++i) {
@@ -282,20 +289,6 @@ bool reparse(int fd, FastxReader &in, const Results &res, size_t n_reads, const 
     }
     if (failed_ok) *failed_ok = second_ok;
     return ok;
-}
-
-}  // namespace
-
-bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf, int failed_fd,
-                       bool *failed_ok) {
-    FastxReader in(path);
-    return reparse(fd, in, res, n_reads, fmt, bgzf, failed_fd, failed_ok);
-}
-
-bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
-                       int failed_fd, bool *failed_ok) {
-    FastxReader in(base, size);
-    return reparse(fd, in, res, n_reads, fmt, bgzf, failed_fd, failed_ok);
 }
 
 bool report_failed_write(const Arguments &args, bool ok) {

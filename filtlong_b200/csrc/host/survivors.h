@@ -16,6 +16,7 @@
 
 #include "../../../include/filtlong_b200.h"
 #include "arguments.h"
+#include "fastx.h"
 
 // Where each record sits in the mapped input, as file offsets. A comment starts one byte after its name (the device and
 // FastxReader both guarantee it).
@@ -79,13 +80,13 @@ inline void append_child_name(std::string &out, const char *name, size_t name_le
 bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want = true);
 bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want = true);
 bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want = true);
-// Sequential: the survivors among the first n_reads records of `path`, parsed again. With failed_fd >= 0 the same parse
-// also writes the other rows to failed_fd (compressed too when bgzf is given), and *failed_ok (when given) tells whether
-// that output was written; the return value is stdout's.
-bool reparse_survivors(int fd, const std::string &path, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
-                       int failed_fd = -1, bool *failed_ok = nullptr);
-// The same over an input held in memory (a stream read once, streamsrc.h)
-bool reparse_survivors(int fd, const char *base, uint64_t size, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
+// Both outputs of a random-access source: the survivors to fd, then, with --failed, the other rows to args.failed_fd (a
+// failure there reported by report_failed_write). True when both were written.
+bool write_outputs(const Arguments &args, int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf);
+// Sequential: the survivors among the first n_reads records of `input` (a path, or bytes in memory), parsed again. With
+// failed_fd >= 0 the same parse also writes the other rows to failed_fd (compressed too when bgzf is given), and
+// *failed_ok (when given) tells whether that output was written; the return value is stdout's.
+bool reparse_survivors(int fd, const FastxInput &input, const Results &res, size_t n_reads, const Format &fmt, fl_ctx *bgzf,
                        int failed_fd = -1, bool *failed_ok = nullptr);
 // --failed: `ok`, after printing an error that names the file when it is false
 bool report_failed_write(const Arguments &args, bool ok);

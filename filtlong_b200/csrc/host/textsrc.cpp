@@ -26,16 +26,16 @@ bool MappedFile::open_plain(const std::string &path) {
     return !gzip;
 }
 
-bool MappedFile::inflate(std::string *why, const GzipDeviceInflate &device) {
+bool MappedFile::inflate(uint64_t budget, std::string *why, const GzipDeviceInflate &device) {
     if (!gzip || !base) return false;
     InflatedInput in;
     int threads = 0;
     if (const char *e = getenv("FL_INFLATE_THREADS")) threads = atoi(e);
-    const bool ok = inflate_gzip_memory((const unsigned char *)base, size, in, threads, 0, why, device);
-    inflater = in.inflater;
+    const bool ok = inflate_gzip_memory((const unsigned char *)base, size, in, threads, budget, why, device);
+    inflater = in.inflater.empty() ? "host threads" : in.inflater;
     if (!ok) return false;
     munmap((void *)base, (size_t)map_bytes);
-    ::close(fd);
+    if (fd >= 0) ::close(fd);
     fd = -1;
     size = in.size;
     map_bytes = in.reserved;
@@ -50,7 +50,7 @@ bool MappedFile::open_any(const std::string &path, bool *inflated, std::string *
     if (!why) why = &w;
     if (!gzip) return false;                                           // not gzip either
     if (getenv("FL_GZ_HOST")) { *why = "FL_GZ_HOST is set"; return false; }
-    if (!inflate(why, device)) return false;                           // declined (gzmem.h)
+    if (!inflate(0, why, device)) return false;                        // declined (gzmem.h)
     if (inflated) *inflated = true;
     return true;
 }
@@ -65,6 +65,12 @@ int MappedFile::format() const {
 MappedFile::~MappedFile() {
     if (base) munmap((void *)base, (size_t)map_bytes);
     if (fd >= 0) ::close(fd);
+}
+
+uint64_t chunk_target(uint64_t default_bytes) {
+    uint64_t target = default_bytes;
+    if (const char *e = getenv("FL_CHUNK_MB")) target = (uint64_t)atoll(e) << 20;
+    return target < (1ull << 20) ? 1ull << 20 : target > (1024ull << 20) ? 1024ull << 20 : target;
 }
 
 namespace {
