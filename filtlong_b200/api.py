@@ -95,7 +95,8 @@ class Context:
     def launch_count(self):
         return int(self.L.fl_ctx_launch_count(self.h))
 
-    KERNELS = {"score_phred": 0, "probe_paint": 1, "kmer_stats": 2, "kmers_add": 3}
+    KERNELS = {"score_phred": 0, "probe_paint": 1, "kmer_stats": 2, "kmers_add": 3,
+               "qual_mask": 4, "row_scan": 5, "qual_gather": 6, "qual_children": 7}
 
     def enable_timing(self, on=True):
         self._ck(self.L.fl_ctx_enable_timing(self.h, int(on)), "fl_ctx_enable_timing")

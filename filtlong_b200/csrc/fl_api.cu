@@ -23,6 +23,7 @@ static int validate_params(const fl_params *p, std::string &why) {
         why = "weight values cannot be negative";                                                                      // arguments.cpp:374-378
         return FL_EINVAL;
     }
+    if (p->trim_q < 0 || p->trim_q > 93) { why = "the value for --trim_q must be an integer from 1 to 93"; return FL_EINVAL; }
     return FL_OK;
 }
 
@@ -396,6 +397,7 @@ extern "C" int fl_reads_push(fl_ctx *c, const fl_batch *h) {
     FL_TRY(check_batch(c, h));
     if (h->n == 0) return fl_score_complete(c);
     if (c->kmers_count_stale || c->multi_pending) FL_TRY(fl_kmers_recount(c));
+    FL_TRY(fl_check_trim_q(c));                                  // before anything is staged
     const bool kmer_mode = c->n_kmers > 0;
     BatchView v{};
     // double-buffered staging: this batch's host->device copies run on the copy stream while the

@@ -181,7 +181,12 @@ struct fl_ctx {
 
     // ---- per-batch scratch ----
     DevVec<uint32_t> sc_pack_seq, sc_pack_nmask;   // 2-bit codes / non-ACGT mask packed on the device from an ASCII DEVICE batch
-    DevVec<uint32_t> sc_mask;        // 1 bit per padded base: base covered by a reference 16-mer
+    DevVec<uint32_t> sc_mask;        // 1 bit per padded base: base covered by a reference 16-mer (or a good 16-run, --trim_q)
+    // --trim_q: the batch's child rows as a view of their own (fl_qtrim.cu): offsets, lengths, gathered quality bytes
+    DevVec<unsigned long long> sc_qoff;
+    DevVec<int32_t> sc_qlen;
+    DevVec<uint8_t> sc_qual;
+    DevVec<unsigned long long> sc_sink;   // fl_phred_pass over rows: the per-read record fields it does not want go here
     DevVec<uint32_t> sc_order;       // rows in descending-length bucket order
     DevVec<uint32_t> tx_nl, tx_u32;  // fl_reads_push_text: newline positions; per-record name / comment / sequence / quality extents
     DevVec<int32_t> sc_items;        // length of each k_kmer_window item: the batch's reads, then its rows
@@ -191,8 +196,10 @@ struct fl_ctx {
     uint32_t *d_buckets = nullptr;         // 256 bucket counters + 256 cursors (fl_order_by_length)
     unsigned long long *d_scalars = nullptr;   // small device scalars (counts, cursors); [30, 39): FL_SCALAR_PHRED_PATHS
     unsigned long long *h_scalars = nullptr;   // pinned mirror
-    // second half of a k-mer batch with --trim / --split, deferred by fl_reads_push (fl_score.cu: score_kmer_back)
+    // second half of a batch with --trim / --split (k-mer mode or --trim_q), deferred by fl_reads_push (fl_score.cu:
+    // score_back)
     bool kmer_pending = false;
+    bool pending_qual = false;              // the deferred batch is a --trim_q batch (no k-mer set)
     BatchView kmer_pending_view{};
     int kmer_pending_slot = -1;             // staging slot to release once the deferred kernels are queued
     cudaEvent_t ev_rows = nullptr;          // the batch's row count has reached h_scalars[FL_HSCALAR_ROWS]
@@ -240,8 +247,8 @@ struct fl_ctx {
     bool timing = false;
     struct TimedLaunch { cudaEvent_t a, b; int which; };
     std::vector<TimedLaunch> timed;
-    double kernel_ms[FL_KERNEL_COUNT] = {0, 0, 0, 0};
-    uint64_t kernel_launches[FL_KERNEL_COUNT] = {0, 0, 0, 0};
+    double kernel_ms[FL_KERNEL_COUNT] = {};
+    uint64_t kernel_launches[FL_KERNEL_COUNT] = {};
 
     void set_error(const std::string &m) { err = m; }
 };
@@ -289,11 +296,29 @@ int fl_kmers_recount(fl_ctx *ctx);
 // that the one host round trip of --trim / --split (how many rows did this batch make?) does not stall the copy pipeline
 int fl_score_view(fl_ctx *ctx, const BatchView &b, bool defer = false);
 int fl_score_complete(fl_ctx *ctx);
+// FL_EINVAL (with a message) when --trim_q is set and the k-mer set is not empty
+int fl_check_trim_q(fl_ctx *ctx);
 int fl_reserve_reads(fl_ctx *ctx, size_t n_total);
 int fl_reserve_rows(fl_ctx *ctx, size_t n_total);
 
 // ---- implemented in fl_phred.cu ----
 int fl_score_phred(fl_ctx *ctx, const BatchView &b);
+// Where one Phred pass writes its scores: mean / window / passed per item of the view, which is a batch's reads or its
+// rows. whole_reads = the items are the context's next reads: also write the rest of each read's record and its
+// identity row (plain Phred mode).
+struct PhredOut {
+    double *mean, *window;
+    uint8_t *passed;
+    bool whole_reads;
+};
+int fl_phred_pass(fl_ctx *ctx, const BatchView &b, const PhredOut &o);
+
+// ---- implemented in fl_qtrim.cu (--trim_q: --trim / --split on Phred qualities) ----
+// sc_mask = 1 bit per padded base: the base lies in a run of FL_K bases whose qualities are all >= 33 + trim_q
+int fl_qual_mask(fl_ctx *ctx, const BatchView &b);
+// the batch's rows [n_rows, n_rows + n_rows_batch) have parent / start / end: score the children on their own quality
+// bytes, give every childless read's row its read's scores
+int fl_score_qual_rows(fl_ctx *ctx, const BatchView &b, size_t n_rows_batch);
 
 // ---- implemented in fl_comm.cu (no-ops / plain copies on a context without a communicator) ----
 int fl_comm_allgather(fl_ctx *ctx, const void *send, void *recv, size_t bytes_per_rank);

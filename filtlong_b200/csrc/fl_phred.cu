@@ -51,7 +51,7 @@ struct PhredArgs {
     uint32_t n;
     const double *lut;          // [512]
     fl_params p;
-    // outputs, already offset to this batch's first read / row
+    // outputs, already offset to this batch's first read / row (or the view's first item: phred_args_of)
     int32_t *r_len, *r_first, *r_last, *r_nbad, *r_nchild;
     double *r_mean, *r_window;
     uint8_t *r_passed;
@@ -1037,32 +1037,62 @@ static int ensure_lut(fl_ctx *ctx) {
     return FL_OK;
 }
 
+// The arguments every Phred kernel shares: the view, the tables and where the scores go. A pass that is not over whole
+// reads sends everything but mean / window / passed to sc_sink, which nothing reads: the kernels stay exactly as they
+// are (a test for the case inside write_read cost k_phred_win<8> a register spill).
+static int phred_args_of(fl_ctx *ctx, const BatchView &b, const PhredOut &o, PhredArgs *out) {
+    PhredArgs a{};
+    a.qual = b.qual; a.off = b.off; a.len = b.len; a.n = b.n;
+    a.lut = ctx->d_lut; a.p = ctx->p;
+    a.r_mean = o.mean; a.r_window = o.window; a.r_passed = o.passed;
+    if (o.whole_reads) {
+        const size_t rb = ctx->n_reads, wb = ctx->n_rows;
+        a.r_len = ctx->r_len.p + rb; a.r_first = ctx->r_first.p + rb; a.r_last = ctx->r_last.p + rb;
+        a.r_nbad = ctx->r_nbad.p + rb; a.r_nchild = ctx->r_nchild.p + rb;
+        a.r_rowstart = ctx->r_rowstart.p + rb;
+        a.w_parent = ctx->w_parent.p + wb; a.w_start = ctx->w_start.p + wb; a.w_end = ctx->w_end.p + wb;
+        a.w_mean = ctx->w_mean.p + wb; a.w_window = ctx->w_window.p + wb; a.w_passed = ctx->w_passed.p + wb;
+        a.read_base = rb; a.row_base = wb;
+    } else {
+        FL_CUDA(ctx, ctx->sc_sink.reserve((size_t)b.n + 1, 0, ctx->stream));   // 8 bytes per item: room for any field
+        unsigned long long *s = ctx->sc_sink.p;
+        int32_t *s32 = reinterpret_cast<int32_t *>(s);
+        a.r_len = a.r_first = a.r_last = a.r_nbad = a.r_nchild = a.w_start = a.w_end = s32;
+        a.r_rowstart = s;
+        a.w_parent = reinterpret_cast<uint32_t *>(s);
+        a.w_mean = a.w_window = reinterpret_cast<double *>(s);
+        a.w_passed = reinterpret_cast<uint8_t *>(s);
+    }
+    *out = a;
+    return FL_OK;
+}
+
 int fl_score_phred(fl_ctx *ctx, const BatchView &b) {
     if (!b.qual) {
         ctx->set_error("FASTA input not supported without an external reference (no quality string and the k-mer set is empty)");
         return FL_EINVAL;                                   // main.cpp:103-106
     }
+    const size_t n = b.n;
+    FL_TRY(fl_reserve_reads(ctx, ctx->n_reads + n));
+    FL_TRY(fl_reserve_rows(ctx, ctx->n_rows + n));
+    const size_t rb = ctx->n_reads;
+    FL_TRY(fl_phred_pass(ctx, b, PhredOut{ctx->r_mean.p + rb, ctx->r_window.p + rb, ctx->r_passed.p + rb, true}));
+    ctx->n_reads += n;
+    ctx->n_rows += n;
+    return FL_OK;
+}
+
+int fl_phred_pass(fl_ctx *ctx, const BatchView &b, const PhredOut &o) {
     FL_TRY(ensure_lut(ctx));
     const size_t n = b.n;
     cudaStream_t st = ctx->stream;
-    FL_TRY(fl_reserve_reads(ctx, ctx->n_reads + n));
-    FL_TRY(fl_reserve_rows(ctx, ctx->n_rows + n));
     const int ws = ctx->p.window_size;
     if (ctx->phred_mode != 0 && ws >= 16 && ws <= 256) {
         // default: one warp per read, both chains by exact grid arithmetic (k_phred_sum, k_phred_win)
         FL_CUDA(ctx, ctx->sc_order.reserve(n, 0, st));
         FL_TRY(fl_order_by_length(ctx, b.len, n, ctx->sc_order.p));
-        PhredArgs a{};
-        a.qual = b.qual; a.off = b.off; a.len = b.len; a.n = b.n;
-        a.lut = ctx->d_lut; a.p = ctx->p;
-        const size_t rb = ctx->n_reads, wb = ctx->n_rows;
-        a.r_len = ctx->r_len.p + rb; a.r_first = ctx->r_first.p + rb; a.r_last = ctx->r_last.p + rb;
-        a.r_nbad = ctx->r_nbad.p + rb; a.r_nchild = ctx->r_nchild.p + rb;
-        a.r_mean = ctx->r_mean.p + rb; a.r_window = ctx->r_window.p + rb; a.r_passed = ctx->r_passed.p + rb;
-        a.r_rowstart = ctx->r_rowstart.p + rb;
-        a.w_parent = ctx->w_parent.p + wb; a.w_start = ctx->w_start.p + wb; a.w_end = ctx->w_end.p + wb;
-        a.w_mean = ctx->w_mean.p + wb; a.w_window = ctx->w_window.p + wb; a.w_passed = ctx->w_passed.p + wb;
-        a.read_base = rb; a.row_base = wb;
+        PhredArgs a;
+        FL_TRY(phred_args_of(ctx, b, o, &a));
         a.order = ctx->sc_order.p;
         a.head_len = (ws + 15) & ~15;                     // k_phred_first sums up to here; k_phred_sum takes over (16-byte loads)
         FL_CUDA(ctx, ctx->sc_f64.reserve(3 * n + 8, 0, st));
@@ -1111,8 +1141,6 @@ int fl_score_phred(fl_ctx *ctx, const BatchView &b) {
         k_phred_fallback<<<ctx->sm_count, PH_THREADS, PH_SMEM, st>>>(a);   // reads the window kernel rejected (normally none)
         ctx->launches++;
         FL_CUDA(ctx, cudaGetLastError());
-        ctx->n_reads += n;
-        ctx->n_rows += n;
         return FL_OK;
     }
     // ---- phred_mode 0 (kept for comparison): work items, one thread per chain ----
@@ -1137,17 +1165,8 @@ int fl_score_phred(fl_ctx *ctx, const BatchView &b) {
     FL_CUDA(ctx, cudaMemsetAsync(fallback, 0, sizeof(uint32_t), st));
     FL_TRY(fl_order_by_key(ctx, cost, n_items, ctx->sc_order.p));
 
-    PhredArgs a{};
-    a.qual = b.qual; a.off = b.off; a.len = b.len; a.n = b.n;
-    a.lut = ctx->d_lut; a.p = ctx->p;
-    const size_t rb = ctx->n_reads, wb = ctx->n_rows;
-    a.r_len = ctx->r_len.p + rb; a.r_first = ctx->r_first.p + rb; a.r_last = ctx->r_last.p + rb;
-    a.r_nbad = ctx->r_nbad.p + rb; a.r_nchild = ctx->r_nchild.p + rb;
-    a.r_mean = ctx->r_mean.p + rb; a.r_window = ctx->r_window.p + rb; a.r_passed = ctx->r_passed.p + rb;
-    a.r_rowstart = ctx->r_rowstart.p + rb;
-    a.w_parent = ctx->w_parent.p + wb; a.w_start = ctx->w_start.p + wb; a.w_end = ctx->w_end.p + wb;
-    a.w_mean = ctx->w_mean.p + wb; a.w_window = ctx->w_window.p + wb; a.w_passed = ctx->w_passed.p + wb;
-    a.read_base = rb; a.row_base = wb;
+    PhredArgs a;
+    FL_TRY(phred_args_of(ctx, b, o, &a));
     a.item_start = ctx->sc_u64a.p; a.order = ctx->sc_order.p; a.items = items; a.n_items = n_items;
     a.it_a = ctx->sc_f64.p; a.it_b = ctx->sc_f64.p + n_items; a.it_c = ctx->sc_f64.p + 2 * n_items;
     a.fallback = fallback;
@@ -1172,7 +1191,5 @@ int fl_score_phred(fl_ctx *ctx, const BatchView &b) {
         ctx->launches += 2;
     }
     FL_CUDA(ctx, cudaGetLastError());
-    ctx->n_reads += n;
-    ctx->n_rows += n;
     return FL_OK;
 }

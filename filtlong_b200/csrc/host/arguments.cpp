@@ -70,6 +70,15 @@ int read_int_suffix(const std::string &name, const std::string &value) {        
     }
 }
 
+// --trim_q (not a reference option): digits only, 1 to 93
+int read_trim_q(const std::string &value) {
+    const size_t digits = value.find_first_not_of('0');
+    const bool ok = !value.empty() && value.find_first_not_of("0123456789") == std::string::npos && digits != std::string::npos &&
+                    value.size() - digits <= 2 && std::stoi(value.substr(digits)) <= 93;
+    if (!ok) throw ParseError("Error: the value for --trim_q must be an integer from 1 to 93");
+    return std::stoi(value.substr(digits));
+}
+
 long long read_plain_ll(const std::string &name, const std::string &value) {         // args.h default reader
     std::istringstream ss(value);
     long long v = 0;
@@ -102,6 +111,7 @@ const Opt kOpts[] = {
     {0, "window_q_weight", true, "float", "weight given to the window quality score (default: 1)"},
     {0, "trim", false, "trim", "trim non-k-mer-matching bases from start/end of reads"},
     {0, "split", true, "split", "split reads at this many (or more) consecutive non-k-mer-matching bases (unit suffixes: k, kb, m, mb, g, gb)"},
+    {0, "trim_q", true, "int", "without a reference, --trim / --split on Phred scores: a base is good if it lies in 16 consecutive bases of at least this quality (1 to 93; not a reference option)"},
     {0, "window_size", true, "int", "size of sliding window used when measuring window quality (default: 250)"},
     {0, "gpus", true, "int", "number of GPUs to shard the read set across (default: 1; not a reference option)"},
     {0, "bgzip", false, "bgzip", "compress the output as BGZF (gzip-compatible) on the GPU (not a reference option)"},
@@ -121,8 +131,8 @@ void print_help(const char *prog) {
         {"output thresholds:", 0, 5},
         {"external references (if provided, read quality will be determined using these instead of from the Phred scores):", 6, 8},
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
-        {"read manipulation:", 12, 13},
-        {"other:", 14, 20},
+        {"read manipulation:", 12, 14},
+        {"other:", 15, 21},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -164,6 +174,7 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "window_q_weight") window_q_weight = read_double(nm, v);
         else if (ln == "trim") trim = true;
         else if (ln == "split") { split = read_int_suffix(nm, v); split_set = true; }
+        else if (ln == "trim_q") trim_q = read_trim_q(v);
         else if (ln == "window_size") window_ll = read_plain_ll(nm, v);
         else if (ln == "gpus") gpus = (int)read_plain_ll(nm, v);
         else if (ln == "bgzip") bgzip = true;
@@ -235,8 +246,10 @@ Arguments::Arguments(int argc, char **argv) {
 #define FAIL(msg) do { fail(msg); return; } while (0)
     if (input_reads.empty()) FAIL("Error: input reads are required");
     const bool some_reference = !short_reads.empty() || assembly_set;
-    if (trim && !some_reference) FAIL("Error: assembly or read reference is required to use --trim");
-    if (split_set && !some_reference) FAIL("Error: assembly or read reference is required to use --split");
+    if (trim_q > 0 && some_reference) FAIL("Error: --trim_q cannot be used with an assembly or read reference");
+    if (trim_q > 0 && !trim && !split_set) FAIL("Error: --trim_q needs --trim or --split");
+    if (trim && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --trim");
+    if (split_set && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --split");
     if (!reads_exist(input_reads)) FAIL("Error: cannot find file: " + input_reads);
     std::vector<std::string> files;
     for (const auto &f : short_reads) files.push_back(f);

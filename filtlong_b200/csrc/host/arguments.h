@@ -39,6 +39,7 @@ public:
     bool trim = false;
     bool split_set = false;
     int split = 0;
+    int trim_q = 0;               // this build only: --trim / --split on Phred qualities without a reference (0 = off)
 
     int window_size = 250;
     bool verbose = false;

@@ -20,6 +20,7 @@ fl_params params_from_arguments(const Arguments &a) {
     p.length_weight = a.length_weight; p.mean_q_weight = a.mean_q_weight; p.window_q_weight = a.window_q_weight;
     p.target_bases_set = a.target_bases_set; p.keep_percent_set = a.keep_percent_set;
     p.target_bases = a.target_bases; p.keep_percent = a.keep_percent;
+    p.trim_q = a.trim_q;
     return p;
 }
 

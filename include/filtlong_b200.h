@@ -63,6 +63,11 @@ typedef struct fl_params {
     int32_t target_bases_set, keep_percent_set;  /* arguments.h:57,60 */
     int64_t target_bases;                        /* arguments.h:58 */
     double keep_percent;                         /* arguments.h:61 */
+    /* Not a reference option: 1..93 makes --trim / --split work without a k-mer set. A base is "good" (the
+     * role of "in a reference 16-mer") when it lies in a run of FL_K consecutive bases whose quality bytes are
+     * all >= 33 + trim_q; children are scored on their own quality bytes. 0 = off. A push with trim_q > 0 onto a
+     * context whose k-mer set is not empty is FL_EINVAL. */
+    int32_t trim_q;
 } fl_params;
 
 /* A batch of sequences in the arena layout above. */
@@ -104,7 +109,10 @@ uint64_t fl_ctx_launch_count(const fl_ctx *ctx);
  * events on the launching stream. fl_ctx_kernel_time synchronises and returns the accumulated
  * milliseconds and launch count of one kernel since the last fl_ctx_reset_timing. */
 enum { FL_KERNEL_SCORE_PHRED = 0, FL_KERNEL_PROBE_PAINT = 1, FL_KERNEL_KMER_STATS = 2, FL_KERNEL_KMERS_ADD = 3,
-       FL_KERNEL_COUNT = 4 };
+       /* --trim_q: the quality mask, the two row passes of the mask (with their scan), the gather of the children's
+        * quality bytes, and the Phred pass over the children (its kernels also count in FL_KERNEL_SCORE_PHRED) */
+       FL_KERNEL_QUAL_MASK = 4, FL_KERNEL_ROW_SCAN = 5, FL_KERNEL_QUAL_GATHER = 6, FL_KERNEL_QUAL_CHILDREN = 7,
+       FL_KERNEL_COUNT = 8 };
 int fl_ctx_enable_timing(fl_ctx *ctx, int on);
 int fl_ctx_reset_timing(fl_ctx *ctx);
 int fl_ctx_kernel_time(fl_ctx *ctx, int which, double *total_ms, uint64_t *launches);
