@@ -96,7 +96,7 @@ class Context:
         return int(self.L.fl_ctx_launch_count(self.h))
 
     KERNELS = {"score_phred": 0, "probe_paint": 1, "kmer_stats": 2, "kmers_add": 3,
-               "qual_mask": 4, "row_scan": 5, "qual_gather": 6, "qual_children": 7}
+               "qual_mask": 4, "row_scan": 5, "qual_gather": 6, "qual_children": 7, "contam": 8}
 
     def enable_timing(self, on=True):
         self._ck(self.L.fl_ctx_enable_timing(self.h, int(on)), "fl_ctx_enable_timing")
@@ -161,6 +161,44 @@ class Context:
         info = (C.c_int32 * 4)()
         self._ck(self.L.fl_kmers_probe_info(self.h, info), "fl_kmers_probe_info")
         return dict(pre_filter=bool(info[0]), filter_kind=int(info[1]), filter_log2_words=int(info[2]), anchored=bool(info[3]))
+
+    # ---- contaminant set (--contam) ----
+    def contam_add(self, seqs, chunk=200000):
+        for i in range(0, len(seqs), chunk):
+            hb = HostBatch(seqs[i:i + chunk], None, want_seq=True, want_nmask=True)
+            b = hb.c_batch()
+            self._ck(self.L.fl_contam_add_batch(self.h, C.byref(b)), "fl_contam_add_batch")
+
+    def contam_add_text(self, data: bytes, fastq=True, is_last=True):
+        """fl_contam_add_text on one chunk of a contaminant file (FASTQ / FASTA text)."""
+        n, nb, used, st = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_int()
+        buf = np.frombuffer(data, dtype=np.uint8)
+        self._ck(self.L.fl_contam_add_text(self.h, capi.ptr(buf), len(data), 1 if fastq else 2, int(is_last),
+                                           C.byref(n), C.byref(nb), C.byref(used), C.byref(st)), "fl_contam_add_text")
+        return dict(status="fallback" if st.value else "ok", n=n.value, bases=nb.value, consumed=used.value)
+
+    def contam_count(self):
+        n = C.c_uint64()
+        self._ck(self.L.fl_contam_finalize(self.h, C.byref(n)), "fl_contam_finalize")
+        return n.value
+
+    def contam_export(self):
+        n = self.contam_count()
+        out = np.zeros(max(n, 1), dtype=np.uint32)
+        got = C.c_uint64()
+        self._ck(self.L.fl_contam_export(self.h, capi.ptr(out), n, C.byref(got)), "fl_contam_export")
+        return out[:n]
+
+    def contam_broadcast(self, root=0):
+        self._ck(self.L.fl_contam_broadcast(self.h, root), "fl_contam_broadcast")
+
+    def contam_results(self):
+        """Per input read: (percent of bases in contaminant 16-mers, removed), and the removed reads / bases / rows."""
+        n, _, _ = self.counts()
+        pct, rem = np.zeros(max(n, 1)), np.zeros(max(n, 1), np.uint8)
+        cc = capi.ContamCounts()
+        self._ck(self.L.fl_results_contam(self.h, capi.ptr(pct), capi.ptr(rem), C.byref(cc)), "fl_results_contam")
+        return pct[:n], rem[:n].astype(bool), dict(reads=cc.reads, bases=cc.bases, rows=cc.rows)
 
     # ---- sharded read set (one context per GPU, NCCL behind the C ABI) ----
     @staticmethod

@@ -34,14 +34,16 @@ class Params(C.Structure):
         ("target_bases", C.c_int64),
         ("keep_percent", C.c_double),
         ("trim_q", C.c_int32),
+        ("max_contam", C.c_double),
     ]
 
 
 def make_params(window_size=250, trim=False, split=None, min_length=None, max_length=None,
                 min_mean_q=None, min_window_q=None, length_weight=1.0, mean_q_weight=1.0,
-                window_q_weight=1.0, target_bases=None, keep_percent=None, trim_q=None):
+                window_q_weight=1.0, target_bases=None, keep_percent=None, trim_q=None, max_contam=50.0):
     """Same keyword surface as the reference CLI options (src/arguments.cpp:152-222), plus `trim_q`
-    (--trim_q: trim / split on Phred qualities when there is no k-mer set; None = off)."""
+    (--trim_q: trim / split on Phred qualities when there is no k-mer set; None = off) and `max_contam`
+    (--max_contam: the removal threshold of the contaminant set, read only when that set is not empty)."""
     p = Params()
     p.window_size = window_size
     p.trim = int(bool(trim))
@@ -61,6 +63,7 @@ def make_params(window_size=250, trim=False, split=None, min_length=None, max_le
     p.keep_percent_set = int(keep_percent is not None)
     p.keep_percent = keep_percent or 0.0
     p.trim_q = trim_q or 0
+    p.max_contam = max_contam
     return p
 
 
@@ -96,6 +99,10 @@ class ReadResults(C.Structure):
 class RowResults(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("parent", "start", "end", "mean_q", "window_q", "length_score",
                                            "norm_mean", "norm_window", "final_score", "passed", "passed_final")]
+
+
+class ContamCounts(C.Structure):
+    _fields_ = [("reads", C.c_uint64), ("bases", C.c_int64), ("rows", C.c_uint64)]
 
 
 class SynthReads(C.Structure):
@@ -145,6 +152,13 @@ SYMBOLS = [
     ("fl_kmers_bitmap_changed", C.c_int, [_P]),
     ("fl_kmers_release_build_state", C.c_int, [_P]),
     ("fl_kmers_probe_info", C.c_int, [_P, C.POINTER(C.c_int32)]),
+    ("fl_contam_add_text", C.c_int, [_P, _P, C.c_uint64, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
+                                     C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
+    ("fl_contam_add_batch", C.c_int, [_P, C.POINTER(Batch)]),
+    ("fl_contam_finalize", C.c_int, [_P, C.POINTER(C.c_uint64)]),
+    ("fl_contam_export", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("fl_contam_broadcast", C.c_int, [_P, C.c_int]),
+    ("fl_results_contam", C.c_int, [_P, _P, _P, C.POINTER(ContamCounts)]),
     ("fl_reads_push", C.c_int, [_P, C.POINTER(Batch)]),
     ("fl_reads_push_text", C.c_int, [_P, _P, C.c_uint64, C.c_int, C.c_int, C.POINTER(TextRecords), C.POINTER(C.c_uint64),
                                      C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),

@@ -97,8 +97,8 @@ extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes,
     if (n_bytes >= ((uint64_t)1 << 31)) { c->set_error("fl_reads_push_bam: a chunk must be smaller than 2 GiB"); return FL_ERANGE; }
     if (n_rec > 0xFFFFFFF0ull) { c->set_error("fl_reads_push_bam: too many records in one chunk"); return FL_ERANGE; }
     if (n_rec == 0) return FL_OK;
-    if (c->kmers_count_stale || c->multi_pending) FL_TRY(fl_kmers_recount(c));
-    const bool kmer_mode = c->n_kmers > 0;
+    FL_TRY(fl_sets_ready(c));
+    const bool kmer_mode = c->ref.n > 0;
     const size_t n = (size_t)n_rec;
     // the arena's layout (padded offsets) and the input's bases (main.cpp:89); every record must lie inside the chunk
     std::vector<uint64_t> off(n);
@@ -141,16 +141,18 @@ extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes,
     v.n = (uint32_t)n; v.padded_bases = padded_bases; v.off = S.off.p; v.len = S.len.p;
     unsigned ggrid = fl_blocks(n * 32, 256);
     if (ggrid > (unsigned)c->sm_count * 16) ggrid = (unsigned)c->sm_count * 16;
-    if (kmer_mode) {
+    if (fl_wants_bases(c)) {                                             // k-mer mode, or a contaminant set to probe
         FL_CUDA(c, S.seq.reserve((size_t)(padded_bases >> 4) + 8, 0, st));
         k_bam_gather<false><<<ggrid, 256, 0, st>>>(S.ascii.p, n_bytes, (uint32_t)n, d_seq_off, d_qual_off, S.len.p, d_off, S.seq.p, nullptr);
         v.seq2b = S.seq.p;
-    } else {
+        c->launches++;
+    }
+    if (!kmer_mode) {
         FL_CUDA(c, S.qual.reserve((size_t)padded_bases + 64, 0, st));
         k_bam_gather<true><<<ggrid, 256, 0, st>>>(S.ascii.p, n_bytes, (uint32_t)n, d_seq_off, d_qual_off, S.len.p, d_off, nullptr, S.qual.p);
         v.qual = S.qual.p;
+        c->launches++;
     }
-    c->launches++;
     FL_CUDA(c, cudaGetLastError());
     FL_TRY(fl_score_view(c, v));
     c->total_bases += bases;                                             // main.cpp:89

@@ -143,19 +143,28 @@ extern "C" int fl_comm_allreduce_i64_host(fl_ctx *ctx, int64_t *inout, int n) {
     return FL_OK;
 }
 
-// Kmers replicated across the shards: the finished direct-address bitmap (512 MiB) goes from `root` to
-// every other rank over NVLink; each rank then derives its own probe tables from it (fl_kmers_recount).
-extern "C" int fl_kmers_broadcast(fl_ctx *ctx, int root) {
-    FL_ENTER(ctx);
-    if (root < 0 || root >= ctx->comm_nranks) { ctx->set_error("fl_kmers_broadcast: bad root"); return FL_EINVAL; }
-    if (ctx->comm_rank == root && (ctx->kmers_count_stale || ctx->multi_pending)) FL_TRY(fl_kmers_recount(ctx));
-    FL_TRY(fl_kmers_ensure_bitmap(ctx));
+// A set replicated across the shards: the finished direct-address bitmap (512 MiB) goes from `root` to every other rank
+// over NVLink; each rank then derives its own probe tables from it (fl_kmers_recount).
+static int broadcast_set(fl_ctx *ctx, KmerSet &s, int root, const char *entry) {
+    if (root < 0 || root >= ctx->comm_nranks) { ctx->set_error(std::string(entry) + ": bad root"); return FL_EINVAL; }
+    if (ctx->comm_rank == root && (s.stale || (&s == &ctx->ref && ctx->multi_pending))) FL_TRY(fl_kmers_recount(ctx, s));
+    FL_TRY(fl_kmers_ensure_bitmap(ctx, s));
     if (!ctx->comm) return FL_OK;
-    FL_NCCL(ctx, nccl().Broadcast(ctx->d_bitmap, ctx->d_bitmap, (size_t)1 << 29, ncclUint8, root, static_cast<ncclComm_t>(ctx->comm),
+    FL_NCCL(ctx, nccl().Broadcast(s.bitmap, s.bitmap, (size_t)1 << 29, ncclUint8, root, static_cast<ncclComm_t>(ctx->comm),
                                   ctx->stream));
     ctx->collectives++;
-    if (ctx->comm_rank != root) ctx->kmers_count_stale = true;
+    if (ctx->comm_rank != root) s.stale = true;
     return FL_OK;
+}
+
+extern "C" int fl_kmers_broadcast(fl_ctx *ctx, int root) {
+    FL_ENTER(ctx);
+    return broadcast_set(ctx, ctx->ref, root, "fl_kmers_broadcast");
+}
+
+extern "C" int fl_contam_broadcast(fl_ctx *ctx, int root) {
+    FL_ENTER(ctx);
+    return broadcast_set(ctx, ctx->contam, root, "fl_contam_broadcast");
 }
 
 extern "C" uint64_t fl_comm_collective_count(const fl_ctx *ctx) { return ctx ? ctx->collectives : 0; }

@@ -246,10 +246,10 @@ __global__ void k_contains(const uint32_t *__restrict__ bm, const uint32_t *__re
 
 }  // namespace
 
-int fl_kmers_ensure_bitmap(fl_ctx *ctx) {
-    if (ctx->d_bitmap) return FL_OK;
-    FL_CUDA(ctx, cudaMalloc(&ctx->d_bitmap, (size_t)1 << 29));
-    FL_CUDA(ctx, cudaMemsetAsync(ctx->d_bitmap, 0, (size_t)1 << 29, ctx->stream));
+int fl_kmers_ensure_bitmap(fl_ctx *ctx, KmerSet &s) {
+    if (s.bitmap) return FL_OK;
+    FL_CUDA(ctx, cudaMalloc(&s.bitmap, (size_t)1 << 29));
+    FL_CUDA(ctx, cudaMemsetAsync(s.bitmap, 0, (size_t)1 << 29, ctx->stream));
     return FL_OK;
 }
 
@@ -284,10 +284,10 @@ static int ensure_multi_state(fl_ctx *ctx) {
     return FL_OK;
 }
 
-int fl_kmers_add_view(fl_ctx *ctx, const BatchView &b, int multi) {
+int fl_kmers_add_view(fl_ctx *ctx, KmerSet &s, const BatchView &b, int multi) {
     if (b.n == 0) return FL_OK;
     if (!b.seq2b) { ctx->set_error("fl_kmers_add_batch: seq2b is required"); return FL_EINVAL; }
-    FL_TRY(fl_kmers_ensure_bitmap(ctx));
+    FL_TRY(fl_kmers_ensure_bitmap(ctx, s));
     if (multi) FL_TRY(ensure_multi_state(ctx));
     size_t n = b.n;
     FL_CUDA(ctx, ctx->sc_u64a.reserve(n + 1, 0, ctx->stream));
@@ -307,7 +307,7 @@ int fl_kmers_add_view(fl_ctx *ctx, const BatchView &b, int multi) {
     BuildArgs a{};
     a.seq2b = b.seq2b; a.nmask = b.nmask; a.off = b.off; a.len = b.len;
     a.tile_start = ctx->sc_u64a.p; a.add_start = ctx->sc_u64b.p;
-    a.n = b.n; a.n_tiles = n_tiles; a.bitmap = ctx->d_bitmap;
+    a.n = b.n; a.n_tiles = n_tiles; a.bitmap = s.bitmap;
     a.seen0 = ctx->d_seen[0]; a.seen1 = ctx->d_seen[1]; a.seen2 = ctx->d_seen[2]; a.seen3 = ctx->d_seen[3];
     a.tfirst = ctx->d_tfirst; a.add_base = ctx->add_counter;
     unsigned long long warps_needed = n_tiles;
@@ -325,93 +325,81 @@ int fl_kmers_add_view(fl_ctx *ctx, const BatchView &b, int multi) {
         ctx->add_counter += n_adds;
         ctx->multi_pending = true;
     }
-    ctx->kmers_count_stale = true;
+    s.stale = true;
     return FL_OK;
 }
 
-int fl_kmers_recount(fl_ctx *ctx) {
-    if (!ctx->d_bitmap) { ctx->n_kmers = 0; ctx->kmers_count_stale = false; return FL_OK; }
-    if (ctx->multi_pending) {
+int fl_kmers_recount(fl_ctx *ctx, KmerSet &s) {
+    if (!s.bitmap) { s.n = 0; s.stale = false; return FL_OK; }
+    if (ctx->multi_pending && &s == &ctx->ref) {
         unsigned blocks = (unsigned)ctx->sm_count * 16;
         k_bloom_times<<<blocks, 256, 0, ctx->stream>>>(ctx->d_seen[0], ctx->d_tfirst, ctx->d_bittime);
-        k_promote<<<blocks, 256, 0, ctx->stream>>>(ctx->d_seen[2], ctx->d_seen[3], ctx->d_tfirst, ctx->d_bittime, ctx->d_bitmap);
+        k_promote<<<blocks, 256, 0, ctx->stream>>>(ctx->d_seen[2], ctx->d_seen[3], ctx->d_tfirst, ctx->d_bittime, s.bitmap);
         ctx->launches += 2;
         ctx->multi_pending = false;
     }
     FL_CUDA(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(unsigned long long), ctx->stream));
-    k_popcount<<<(unsigned)ctx->sm_count * 8, 256, 0, ctx->stream>>>(ctx->d_bitmap, (size_t)1 << 27, ctx->d_scalars);
+    k_popcount<<<(unsigned)ctx->sm_count * 8, 256, 0, ctx->stream>>>(s.bitmap, (size_t)1 << 27, ctx->d_scalars);
     ctx->launches++;
     FL_CUDA(ctx, cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
     FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->n_kmers = ctx->h_scalars[0];
-    ctx->kmers_count_stale = false;
+    s.n = ctx->h_scalars[0];
+    s.stale = false;
     // The pre-filter is used while it has filter_min_bits_per_key bits per member (fl_internal.cuh: on the H100 a 20 M-member
     // set probes faster without it). Larger sets (config 3's, or a 3 Gbp assembly that fills 75 % of the key space) are
     // probed directly.
     const size_t filter_words = (size_t)1 << ctx->filter_log2_words;
-    ctx->use_filter = ctx->filter_enabled && ctx->n_kmers > 0 && ctx->n_kmers * (uint64_t)ctx->filter_min_bits_per_key <= filter_words * 64;
+    s.use_filter = ctx->filter_enabled && s.n > 0 && s.n * (uint64_t)ctx->filter_min_bits_per_key <= filter_words * 64;
     // Which flavour: the probe kernel is bound by L1TEX sector look-ups on a sparse set, one per filter word it loads, so a
     // word shared by the four 16-mers of a table group (or by two neighbours) cuts them 4x (2x) -- at 4x (2x) the insertions.
     // Small sets can afford that (false positives, each a wasted random HBM sector, stay below ~5 %); the thresholds
     // (filter_group4_max, filter_pair_max) come from a sweep of config 3's reads against sets of 5 to 20 M members.
-    if (ctx->filter_kind_request >= 0) ctx->filter_kind = ctx->filter_kind_request;
-    else if (!ctx->anchor_enabled) ctx->filter_kind = 2 | 16;
-    else if (ctx->n_kmers <= ctx->filter_group4_max) ctx->filter_kind = 2 | 4 | 16;
-    else if (ctx->n_kmers <= ctx->filter_pair_max) ctx->filter_kind = 2 | 8 | 16;
-    else ctx->filter_kind = 2 | 16;
-    if (!ctx->anchor_enabled) ctx->filter_kind &= ~(4 | 8);        // the keyed flavours follow the anchored table's groups
-    if (ctx->use_filter) {
-        if (!ctx->d_filter) FL_CUDA(ctx, cudaMalloc(&ctx->d_filter, filter_words * sizeof(unsigned long long)));
-        FL_CUDA(ctx, cudaMemsetAsync(ctx->d_filter, 0, filter_words * sizeof(unsigned long long), ctx->stream));
-        k_filter_build<<<(unsigned)ctx->sm_count * 16, 256, 0, ctx->stream>>>(ctx->d_bitmap, ctx->d_filter, ctx->filter_log2_words, ctx->filter_kind);
+    if (ctx->filter_kind_request >= 0) s.filter_kind = ctx->filter_kind_request;
+    else if (!ctx->anchor_enabled) s.filter_kind = 2 | 16;
+    else if (s.n <= ctx->filter_group4_max) s.filter_kind = 2 | 4 | 16;
+    else if (s.n <= ctx->filter_pair_max) s.filter_kind = 2 | 8 | 16;
+    else s.filter_kind = 2 | 16;
+    if (!ctx->anchor_enabled) s.filter_kind &= ~(4 | 8);        // the keyed flavours follow the anchored table's groups
+    if (s.use_filter) {
+        if (!s.filter) FL_CUDA(ctx, cudaMalloc(&s.filter, filter_words * sizeof(unsigned long long)));
+        FL_CUDA(ctx, cudaMemsetAsync(s.filter, 0, filter_words * sizeof(unsigned long long), ctx->stream));
+        k_filter_build<<<(unsigned)ctx->sm_count * 16, 256, 0, ctx->stream>>>(s.bitmap, s.filter, ctx->filter_log2_words, s.filter_kind);
         ctx->launches++;
         FL_CUDA(ctx, cudaGetLastError());
     }
     // the table the probe kernel reads: one 32-byte sector per four consecutive 16-mers of a read
-    ctx->use_anchor = ctx->anchor_enabled && ctx->n_kmers > 0;
-    if (ctx->use_anchor) {
+    s.use_anchor = ctx->anchor_enabled && s.n > 0;
+    if (s.use_anchor) {
         const size_t anchor_bytes = (size_t)1 << 31;
-        if (!ctx->d_anchor) FL_CUDA(ctx, cudaMalloc(&ctx->d_anchor, anchor_bytes));
-        FL_CUDA(ctx, cudaMemsetAsync(ctx->d_anchor, 0, anchor_bytes, ctx->stream));
-        k_anchor_build<<<(unsigned)ctx->sm_count * 16, 256, 0, ctx->stream>>>(ctx->d_bitmap, ctx->d_anchor);
+        if (!s.anchor) FL_CUDA(ctx, cudaMalloc(&s.anchor, anchor_bytes));
+        FL_CUDA(ctx, cudaMemsetAsync(s.anchor, 0, anchor_bytes, ctx->stream));
+        k_anchor_build<<<(unsigned)ctx->sm_count * 16, 256, 0, ctx->stream>>>(s.bitmap, s.anchor);
         ctx->launches++;
         FL_CUDA(ctx, cudaGetLastError());
     }
     return FL_OK;
 }
 
-// ---- C ABI ------------------------------------------------------------------------------------
-extern "C" int fl_kmers_finalize(fl_ctx *ctx, uint64_t *n_kmers_out) {
-    FL_ENTER(ctx);
-    if (ctx->kmers_count_stale || ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx));
-    if (n_kmers_out) *n_kmers_out = ctx->n_kmers;
+int fl_sets_ready(fl_ctx *ctx) {
+    if (ctx->ref.stale || ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx, ctx->ref));
+    if (ctx->contam.stale) FL_TRY(fl_kmers_recount(ctx, ctx->contam));
     return FL_OK;
 }
 
-extern "C" int fl_kmers_contains(fl_ctx *ctx, const uint32_t *kmers, uint32_t n, uint8_t *out) {
-    if (!ctx || (!kmers && n) || (!out && n)) return FL_EINVAL;
-    FL_ENTER(ctx);
-    FL_TRY(fl_kmers_finalize(ctx, nullptr));
-    if (n == 0) return FL_OK;
-    if (!ctx->d_bitmap) { memset(out, 0, n); return FL_OK; }
-    FL_CUDA(ctx, ctx->sc_u32a.reserve((size_t)n + (n + 3) / 4, 0, ctx->stream));
-    uint32_t *dq = ctx->sc_u32a.p;
-    uint8_t *dout = reinterpret_cast<uint8_t *>(dq + n);
-    FL_CUDA(ctx, cudaMemcpyAsync(dq, kmers, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    k_contains<<<fl_blocks(n, 256), 256, 0, ctx->stream>>>(ctx->d_bitmap, dq, n, dout);
-    ctx->launches++;
-    FL_CUDA(ctx, cudaMemcpyAsync(out, dout, n, cudaMemcpyDeviceToHost, ctx->stream));
-    FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+int fl_contam_check_order(fl_ctx *ctx) {
+    if (ctx->n_reads > 0 || ctx->kmer_pending) {
+        ctx->set_error("the contaminant set must be built before any read is pushed (fl_reads_reset first)");
+        return FL_EINVAL;
+    }
     return FL_OK;
 }
 
-extern "C" int fl_kmers_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out) {
-    FL_ENTER(ctx);
-    FL_TRY(fl_kmers_finalize(ctx, nullptr));
-    if (n_out) *n_out = ctx->n_kmers;
-    if (!ctx->d_bitmap || !out || cap == 0) return FL_OK;
+// the set's members in ascending order (at most cap of them)
+static int export_set(fl_ctx *ctx, KmerSet &s, uint32_t *out, uint64_t cap, uint64_t *n_out) {
+    if (n_out) *n_out = s.n;
+    if (!s.bitmap || !out || cap == 0) return FL_OK;
     std::vector<uint32_t> host((size_t)1 << 27);
-    FL_CUDA(ctx, cudaMemcpyAsync(host.data(), ctx->d_bitmap, (size_t)1 << 29, cudaMemcpyDeviceToHost, ctx->stream));
+    FL_CUDA(ctx, cudaMemcpyAsync(host.data(), s.bitmap, (size_t)1 << 29, cudaMemcpyDeviceToHost, ctx->stream));
     FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     uint64_t k = 0;
     for (size_t w = 0; w < host.size() && k < cap; ++w) {
@@ -425,36 +413,81 @@ extern "C" int fl_kmers_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_
     return FL_OK;
 }
 
+// ---- C ABI ------------------------------------------------------------------------------------
+extern "C" int fl_kmers_finalize(fl_ctx *ctx, uint64_t *n_kmers_out) {
+    FL_ENTER(ctx);
+    if (ctx->ref.stale || ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx, ctx->ref));
+    if (n_kmers_out) *n_kmers_out = ctx->ref.n;
+    return FL_OK;
+}
+
+extern "C" int fl_kmers_contains(fl_ctx *ctx, const uint32_t *kmers, uint32_t n, uint8_t *out) {
+    if (!ctx || (!kmers && n) || (!out && n)) return FL_EINVAL;
+    FL_ENTER(ctx);
+    FL_TRY(fl_kmers_finalize(ctx, nullptr));
+    if (n == 0) return FL_OK;
+    if (!ctx->ref.bitmap) { memset(out, 0, n); return FL_OK; }
+    FL_CUDA(ctx, ctx->sc_u32a.reserve((size_t)n + (n + 3) / 4, 0, ctx->stream));
+    uint32_t *dq = ctx->sc_u32a.p;
+    uint8_t *dout = reinterpret_cast<uint8_t *>(dq + n);
+    FL_CUDA(ctx, cudaMemcpyAsync(dq, kmers, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    k_contains<<<fl_blocks(n, 256), 256, 0, ctx->stream>>>(ctx->ref.bitmap, dq, n, dout);
+    ctx->launches++;
+    FL_CUDA(ctx, cudaMemcpyAsync(out, dout, n, cudaMemcpyDeviceToHost, ctx->stream));
+    FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return FL_OK;
+}
+
+extern "C" int fl_kmers_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out) {
+    FL_ENTER(ctx);
+    FL_TRY(fl_kmers_finalize(ctx, nullptr));
+    return export_set(ctx, ctx->ref, out, cap, n_out);
+}
+
 extern "C" int fl_kmers_bitmap_dev(fl_ctx *ctx, void **dev_ptr, uint64_t *n_bytes) {
     if (!ctx || !dev_ptr) return FL_EINVAL;
     FL_ENTER(ctx);
-    FL_TRY(fl_kmers_ensure_bitmap(ctx));
-    *dev_ptr = ctx->d_bitmap;
+    FL_TRY(fl_kmers_ensure_bitmap(ctx, ctx->ref));
+    *dev_ptr = ctx->ref.bitmap;
     if (n_bytes) *n_bytes = (uint64_t)1 << 29;
     return FL_OK;
 }
 
 extern "C" int fl_kmers_bitmap_changed(fl_ctx *ctx) {
     FL_ENTER(ctx);
-    ctx->kmers_count_stale = true;
+    ctx->ref.stale = true;
     return FL_OK;
 }
 
 extern "C" int fl_kmers_probe_info(fl_ctx *ctx, int32_t info[4]) {
     FL_ENTER(ctx);
     if (!info) return FL_EINVAL;
-    if (ctx->kmers_count_stale || ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx));
-    info[0] = ctx->use_filter ? 1 : 0;
-    info[1] = ctx->filter_kind;
+    if (ctx->ref.stale || ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx, ctx->ref));
+    info[0] = ctx->ref.use_filter ? 1 : 0;
+    info[1] = ctx->ref.filter_kind;
     info[2] = (int32_t)ctx->filter_log2_words;
-    info[3] = ctx->use_anchor ? 1 : 0;
+    info[3] = ctx->ref.use_anchor ? 1 : 0;
     return FL_OK;
 }
 
 extern "C" int fl_kmers_release_build_state(fl_ctx *ctx) {
     FL_ENTER(ctx);
-    if (ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx));
+    if (ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx, ctx->ref));
     FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     free_multi_state(ctx);
     return FL_OK;
+}
+
+// ---- the contaminant set: the reference set's code with assembly semantics (kmers.cpp:137-139) ----
+extern "C" int fl_contam_finalize(fl_ctx *ctx, uint64_t *n_kmers_out) {
+    FL_ENTER(ctx);
+    if (ctx->contam.stale) FL_TRY(fl_kmers_recount(ctx, ctx->contam));
+    if (n_kmers_out) *n_kmers_out = ctx->contam.n;
+    return FL_OK;
+}
+
+extern "C" int fl_contam_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out) {
+    FL_ENTER(ctx);
+    FL_TRY(fl_contam_finalize(ctx, nullptr));
+    return export_set(ctx, ctx->contam, out, cap, n_out);
 }

@@ -31,6 +31,7 @@ struct RowsView {
     const int32_t *start, *end;
     const double *mean, *window;
     const uint8_t *passed;
+    const uint8_t *excl;             // rows of reads removed by the contaminant set (skipped); null without one
 };
 
 __device__ __forceinline__ double warp_sum(double v) {
@@ -60,6 +61,7 @@ __global__ void __launch_bounds__(RED_THREADS) k_norm_p1(RowsView v, double *__r
     const size_t lo = chunk * blockIdx.x, hi = lo + chunk < v.n ? lo + chunk : v.n;
     double s = 0.0, pb = 0.0, rb = 0.0, mn = 100.0, mx = 0.0, cnt = 0.0;   // main.cpp:170-172
     for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+        if (v.excl && v.excl[i]) continue;
         const double x = v.mean[i];
         const double len = (double)(v.end[i] - v.start[i]);
         s += x;
@@ -123,6 +125,7 @@ __global__ void __launch_bounds__(RED_THREADS) k_norm_p2(RowsView v, const doubl
     const size_t lo = chunk * blockIdx.x, hi = lo + chunk < v.n ? lo + chunk : v.n;
     double s = 0.0;
     for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+        if (v.excl && v.excl[i]) continue;
         const double d = v.mean[i] - mean;                                   // main.cpp:182-183
         s += d * d;
     }
@@ -514,6 +517,7 @@ static RowsView rows_view(fl_ctx *c) {
     RowsView v{};
     v.n = c->n_rows;
     v.start = c->w_start.p; v.end = c->w_end.p; v.mean = c->w_mean.p; v.window = c->w_window.p; v.passed = c->w_passed.p;
+    v.excl = c->contam.n > 0 ? c->w_excl.p : nullptr;
     return v;
 }
 

@@ -109,6 +109,8 @@ const Opt kOpts[] = {
     {0, "length_weight", true, "float", "weight given to the length score (default: 1)"},
     {0, "mean_q_weight", true, "float", "weight given to the mean quality score (default: 1)"},
     {0, "window_q_weight", true, "float", "weight given to the window quality score (default: 1)"},
+    {0, "contam", true, "file", "remove reads that come from these sequences (FASTA or FASTQ, may be gzipped), judged by their 16-mers (not a reference option)"},
+    {0, "max_contam", true, "float", "remove a read when more than this percentage of its bases lie in a 16-mer of --contam (default: 50; not a reference option)"},
     {0, "trim", false, "trim", "trim non-k-mer-matching bases from start/end of reads"},
     {0, "split", true, "split", "split reads at this many (or more) consecutive non-k-mer-matching bases (unit suffixes: k, kb, m, mb, g, gb)"},
     {0, "trim_q", true, "int", "without a reference, --trim / --split on Phred scores: a base is good if it lies in 16 consecutive bases of at least this quality (1 to 93; not a reference option)"},
@@ -131,8 +133,9 @@ void print_help(const char *prog) {
         {"output thresholds:", 0, 5},
         {"external references (if provided, read quality will be determined using these instead of from the Phred scores):", 6, 8},
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
-        {"read manipulation:", 12, 14},
-        {"other:", 15, 21},
+        {"contaminant removal:", 12, 13},
+        {"read manipulation:", 14, 16},
+        {"other:", 17, 23},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -172,6 +175,8 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "length_weight") length_weight = read_double(nm, v);
         else if (ln == "mean_q_weight") mean_q_weight = read_double(nm, v);
         else if (ln == "window_q_weight") window_q_weight = read_double(nm, v);
+        else if (ln == "contam") { contam = v; contam_set = true; }
+        else if (ln == "max_contam") { max_contam = read_double(nm, v); max_contam_set = true; }
         else if (ln == "trim") trim = true;
         else if (ln == "split") { split = read_int_suffix(nm, v); split_set = true; }
         else if (ln == "trim_q") trim_q = read_trim_q(v);
@@ -250,14 +255,19 @@ Arguments::Arguments(int argc, char **argv) {
     if (trim_q > 0 && !trim && !split_set) FAIL("Error: --trim_q needs --trim or --split");
     if (trim && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --trim");
     if (split_set && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --split");
+    if (max_contam_set && !contam_set) FAIL("Error: --max_contam needs --contam");
+    if (contam_set && !(max_contam >= 0.0 && max_contam < 100.0))
+        FAIL("Error: the value for --max_contam must be at least 0 and less than 100");
     if (!reads_exist(input_reads)) FAIL("Error: cannot find file: " + input_reads);
     std::vector<std::string> files;
     for (const auto &f : short_reads) files.push_back(f);
     if (assembly_set) files.push_back(assembly);
+    if (contam_set) files.push_back(contam);
     for (const auto &f : files)
         if (!does_file_exist(f)) FAIL("Error: cannot find file: " + f);
+    // --contam removes reads on its own: it counts as a threshold (the message below stays the reference's)
     if (!trim && !split_set && !target_bases_set && !keep_percent_set && !min_length_set && !max_length_set &&
-        !min_mean_q_set && !min_window_q_set)
+        !min_mean_q_set && !min_window_q_set && !contam_set)
         FAIL("Error: no thresholds set, you must use one of the following options:\n"
              "target_bases, keep_percent, min_length, max_length, min_mean_q, min_window_q, trim, split");
     if (target_bases_set && target_bases <= 0) FAIL("Error: the value for --target_bases must be a positive integer");

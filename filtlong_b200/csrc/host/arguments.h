@@ -40,6 +40,11 @@ public:
     bool split_set = false;
     int split = 0;
     int trim_q = 0;               // this build only: --trim / --split on Phred qualities without a reference (0 = off)
+    // this build only: reads with more than max_contam percent of their bases in 16-mers of this file are removed
+    bool contam_set = false;
+    std::string contam;
+    bool max_contam_set = false;
+    double max_contam = 50.0;
 
     int window_size = 250;
     bool verbose = false;

@@ -43,6 +43,7 @@ struct Shard {
     std::vector<uint64_t> row_start;
     std::vector<uint8_t> row_pfinal;
     uint64_t n_rows = 0;
+    fl_contam_counts contam{};                  // --contam: what the shard's reads lost
     fl_summary summary{};
     std::string error;
     bool fallback = false;
@@ -220,7 +221,7 @@ ChunkPush bam_push(const char *base, std::vector<BamChunkIndex> &idx) {
 // readers below are already filling the ring by then)
 void run_shard(Shard &sh, const MappedFile &f, Plan &plan, const ChunkPush &push, const fl_params &params, int nranks,
                const unsigned char *comm_id, const std::function<fl_ctx *()> &get_ctx0, std::atomic<bool> &abort_all, uint64_t slot_bytes,
-               bool share_kmers, StreamInput *stream) {
+               bool share_kmers, bool share_contam, StreamInput *stream) {
     Ring ring;
     if (const char *e = getenv("FL_READERS")) {
         const int k = atoi(e);
@@ -282,6 +283,11 @@ void run_shard(Shard &sh, const MappedFile &f, Plan &plan, const ChunkPush &push
                 uint64_t nk = 0;
                 check(sh.ctx, fl_kmers_finalize(sh.ctx, &nk), "fl_kmers_finalize");
             }
+            if (share_contam) {
+                check(sh.ctx, fl_contam_broadcast(sh.ctx, 0), "fl_contam_broadcast");
+                uint64_t nk = 0;
+                check(sh.ctx, fl_contam_finalize(sh.ctx, &nk), "fl_contam_finalize");
+            }
         }
         size_t guess = 0;
         for (size_t i = 0; i < n_chunks && !abort_all.load(); ++i) {
@@ -340,6 +346,7 @@ void finalize_shard(Shard &sh) {
         fl_row_results wr{};
         wr.start = sh.row_s.data(); wr.end = sh.row_e.data(); wr.passed_final = sh.row_pfinal.data();
         check(sh.ctx, fl_results_rows(sh.ctx, &wr), "fl_results_rows");
+        check(sh.ctx, fl_results_contam(sh.ctx, nullptr, nullptr, &sh.contam), "fl_results_contam");
     } catch (const std::exception &e) {
         sh.error = e.what();
     }
@@ -482,7 +489,7 @@ void plan_stream(StreamInput &stream, int format, const Cuts &cuts, Plan &plan) 
 // Runs every shard, shard 0 on this thread, and a growing stream's planner beside them. true: a shard handed a chunk back,
 // or a stream's plan failed; the host path is then to read the whole input.
 bool score(std::vector<Shard> &shards, const Source &src, const Cuts &cuts, Plan &plan, const ChunkPush &push, const Arguments &args,
-           Kmers &kmers, bool share_kmers) {
+           Kmers &kmers, bool share_kmers, bool share_contam) {
     const int nranks = (int)shards.size();
     unsigned char comm_id[FL_COMM_ID_BYTES] = {0};
     if (nranks > 1 && fl_comm_unique_id(comm_id) != FL_OK) throw std::runtime_error("NCCL is not available: cannot shard across GPUs");
@@ -494,8 +501,9 @@ bool score(std::vector<Shard> &shards, const Source &src, const Cuts &cuts, Plan
     std::vector<std::thread> ts;
     for (int r = 1; r < nranks; ++r)
         ts.emplace_back(run_shard, std::ref(shards[r]), std::cref(*src.file), std::ref(plan), std::cref(push), std::cref(params), nranks, comm_id,
-                        std::cref(get_ctx0), std::ref(abort_all), cuts.max_chunk, share_kmers, src.stream);
-    run_shard(shards[0], *src.file, plan, push, params, nranks, comm_id, get_ctx0, abort_all, cuts.max_chunk, share_kmers, src.stream);
+                        std::cref(get_ctx0), std::ref(abort_all), cuts.max_chunk, share_kmers, share_contam, src.stream);
+    run_shard(shards[0], *src.file, plan, push, params, nranks, comm_id, get_ctx0, abort_all, cuts.max_chunk, share_kmers, share_contam,
+              src.stream);
     for (auto &t : ts) t.join();
     if (planner.joinable()) planner.join();
     return abort_all.load();
@@ -532,8 +540,14 @@ void finalize(std::vector<Shard> &shards, const Arguments &args, const Mark &mar
     throw_shard_error(shards);
     mark("finalize + download");
     uint64_t n_rows = 0;
-    for (auto &s : shards) n_rows += s.n_rows;
+    long long removed_reads = 0, removed_bases = 0;
+    for (auto &s : shards) {
+        n_rows += s.n_rows - s.contam.rows;
+        removed_reads += (long long)s.contam.reads;
+        removed_bases += (long long)s.contam.bases;
+    }
     log_after_trim_split(args, n_rows, shards[0].summary);
+    if (args.contam_set) print_contam_removal(args.max_contam, removed_reads, removed_bases);
     log_filtering(args, shards[0].summary);
 }
 
@@ -553,7 +567,7 @@ FeederOutcome run_device_feeder(Arguments &args, Kmers &kmers, StreamInput *stre
     const ChunkPush push = bam ? bam_push(f.base, bam_idx) : text_push(src.format);
     ShardSet shards(plan.chunks, f.size, args.gpus, src.growing);
     const bool kmers_empty = kmers.empty();
-    const bool declined = score(shards.v, src, cuts, plan, push, args, kmers, !kmers_empty);
+    const bool declined = score(shards.v, src, cuts, plan, push, args, kmers, !kmers_empty, kmers.contam_size() > 0);
     std::string why;
     if (src.growing && !stream->finish(&why)) throw std::runtime_error(why);
     throw_shard_error(shards.v);

@@ -1,6 +1,7 @@
 // filtlong_b200/csrc/host/kmers.cpp -- see kmers.h. Log lines follow reference src/kmers.cpp:50-72.
 #include "kmers.h"
 
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -101,6 +102,28 @@ void Kmers::add_assembly_fasta(std::string filename) {
               << int_to_string((long long)size()) << " 16-mers\n\n";
 }
 
+uint64_t Kmers::contam_size() {
+    if (!ctx_) return 0;
+    uint64_t n = 0;
+    check(ctx_, fl_contam_finalize(ctx_, &n), "fl_contam_finalize");
+    return n;
+}
+
+// The same block as add_assembly_fasta's (kmers.cpp:61-72), then the chance that a base of random sequence lies in one
+// of the set's 16-mers: the 16-mers of a genome the size of a human one cover almost every base, which removes everything.
+void Kmers::add_contaminant_fasta(const std::string &filename) {
+    std::cerr << "Hashing 16-mers from contaminant sequences\n";
+    std::cerr << "  " << filename << "\n";
+    const int sequence_count = add_reference(filename, false, true);
+    const uint64_t n = contam_size();
+    std::cerr << "  " << int_to_string(sequence_count) << " " << (sequence_count == 1 ? "contig" : "contigs") << ", "
+              << int_to_string((long long)n) << " 16-mers\n";
+    const double covered = -expm1(16.0 * log1p(-(double)n / 4294967296.0));      // 1 - (1 - n / 4^16)^16
+    char buf[96];
+    snprintf(buf, sizeof buf, "  a random base lies in one of them with probability %.3g\n\n", covered);
+    std::cerr << buf;
+}
+
 // The reference's loop (kmers.cpp:75-134) parses one record at a time through kseq on the calling thread. Here the file
 // is one byte range (mapped, or a gzip file inflated once: textsrc.h) whose record-aligned chunks go to the device as
 // TEXT (fl_kmers_add_text): records (4-line FASTQ; FASTA with one sequence line or evenly wrapped), validation, 2-bit
@@ -108,7 +131,7 @@ void Kmers::add_assembly_fasta(std::string filename) {
 // lines, a broken record ...) -- and everything after it -- is parsed
 // by the kseq-compatible host reader from that chunk's first byte, so the adds stay in file order and the reader stops
 // where the reference's would (a parse error silently ends hashing: kmers.cpp:90-94).
-int Kmers::add_reference(const std::string &filename, bool multi) {
+int Kmers::add_reference(const std::string &filename, bool multi, bool contam) {
     int sequence_count = 0;
     long long base_count = 0, last_progress = 0;
     auto progress = [&](bool force) {
@@ -125,7 +148,8 @@ int Kmers::add_reference(const std::string &filename, bool multi) {
             if (arena.empty()) return;
             fl_batch b = arena.batch();
             fl_ctx *c = context();
-            check(c, fl_kmers_add_batch(c, &b, multi ? 1 : 0), "fl_kmers_add_batch");
+            if (contam) check(c, fl_contam_add_batch(c, &b), "fl_contam_add_batch");
+            else check(c, fl_kmers_add_batch(c, &b, multi ? 1 : 0), "fl_kmers_add_batch");
             arena.clear();
         };
         while (in.ok() && in.next() >= 0) {        // a parse error silently ends hashing (kmers.cpp:90-94)
@@ -156,8 +180,13 @@ int Kmers::add_reference(const std::string &filename, bool multi) {
             const Chunk &ch = plan[i];
             uint64_t n_rec = 0, n_bases = 0, used = 0;
             int status = FL_TEXT_OK;
-            check(c, fl_kmers_add_text(c, f.base + ch.begin, ch.end - ch.begin, f.format(), i + 1 == plan.size() ? 1 : 0, multi ? 1 : 0,
-                                       &n_rec, &n_bases, &used, &status), "fl_kmers_add_text");
+            const int last = i + 1 == plan.size() ? 1 : 0;
+            if (contam)
+                check(c, fl_contam_add_text(c, f.base + ch.begin, ch.end - ch.begin, f.format(), last, &n_rec, &n_bases, &used, &status),
+                      "fl_contam_add_text");
+            else
+                check(c, fl_kmers_add_text(c, f.base + ch.begin, ch.end - ch.begin, f.format(), last, multi ? 1 : 0, &n_rec, &n_bases, &used,
+                                           &status), "fl_kmers_add_text");
             if (status == FL_TEXT_OK) {                                 // the chunk's whole records (all of it, normally) are in
                 sequence_count += (int)n_rec;
                 base_count += (long long)n_bases;

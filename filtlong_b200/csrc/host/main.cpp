@@ -83,6 +83,7 @@ int main(int argc, char **argv) {
         if (args.assembly_set) kmers.add_assembly_fasta(args.assembly);
         if (!args.short_reads.empty()) kmers.add_read_fastqs(args.short_reads);
         const bool kmers_empty = kmers.empty();
+        if (args.contam_set) kmers.add_contaminant_fasta(args.contam);   // after -1/-2, whose build state is released by now
         timer.mark("reference k-mers (+ CUDA init)");
 
         // ---- the device feeder ----
@@ -121,6 +122,7 @@ int main(int argc, char **argv) {
             if (!args.verbose) return;
             reads.download();
             for (; verbose_done < reads.n_reads(); ++verbose_done) {
+                if (reads.removed[verbose_done]) continue;                // --contam: as if the read were not in the input
                 Read *r = reads.make_read(verbose_done);
                 r->print_verbose_read_info();                             // main.cpp:110-111
                 delete r;
@@ -195,12 +197,15 @@ int main(int argc, char **argv) {
         timer.mark("finalize + download");
         size_t longest_read_name = 0;
         if (args.verbose)
-            for (size_t row = 0; row < reads.n_rows(); ++row) longest_read_name = std::max(longest_read_name, reads.row_name(row).size());
-        log_after_trim_split(args, reads.n_rows(), summary);
+            for (size_t row = 0; row < reads.n_rows(); ++row)
+                if (reads.ranked(row)) longest_read_name = std::max(longest_read_name, reads.row_name(row).size());
+        log_after_trim_split(args, reads.n_rows() - reads.contam.rows, summary);
+        if (args.contam_set) print_contam_removal(args.max_contam, (long long)reads.contam.reads, (long long)reads.contam.bases);
         if (args.verbose) {
             std::cerr << "\n\n" << "Read name" << "\t" << "Length score" << "\t" << "Mean quality score" << "\t"
                       << "Window quality score" << "\t" << "Final score" << "\n";
             for (size_t row = 0; row < reads.n_rows(); ++row) {
+                if (!reads.ranked(row)) continue;                        // a removed read's rows are not ranked
                 std::string nm = reads.row_name(row);
                 if (longest_read_name > nm.size()) nm += std::string(longest_read_name - nm.size(), ' ');
                 std::cerr << nm << "\t" << double_to_string(reads.row_lscore[row]) << "\t" << double_to_string(reads.row_nmean[row])

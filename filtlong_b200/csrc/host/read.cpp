@@ -21,6 +21,7 @@ fl_params params_from_arguments(const Arguments &a) {
     p.target_bases_set = a.target_bases_set; p.keep_percent_set = a.keep_percent_set;
     p.target_bases = a.target_bases; p.keep_percent = a.keep_percent;
     p.trim_q = a.trim_q;
+    p.max_contam = a.max_contam;
     return p;
 }
 
@@ -28,10 +29,12 @@ fl_params params_from_arguments(const Arguments &a) {
 // ReadSet
 // ---------------------------------------------------------------------------------------------
 ReadSet::ReadSet(Kmers *kmers, Arguments *args) : kmers_(kmers), args_(args) {
-    // nothing here touches the GPU: records can be parsed and packed while the CUDA context is still
-    // coming up (Kmers creates it on first use); the parameters are set with the first batch
+    // nothing here waits for the GPU: records can be parsed and packed while the CUDA context is still coming up
+    // (Kmers creates it on first use; both sets are finalised by the time they are asked for their size here); the
+    // parameters are set with the first batch
     kmer_mode_ = !kmers->empty();                          // read.cpp:35
-    arena_ = new HostArena(kmer_mode_, !kmer_mode_, false);
+    // the bases are packed in k-mer mode, and for the contaminant set's probe
+    arena_ = new HostArena(kmer_mode_ || kmers->contam_size() > 0, !kmer_mode_, false);
 }
 
 fl_ctx *ReadSet::ready_context() {
@@ -86,6 +89,8 @@ void ReadSet::download() {
     wr.norm_mean = row_nmean.data(); wr.norm_window = row_nwindow.data(); wr.final_score = row_final.data();
     wr.passed = row_passed.data(); wr.passed_final = row_pfinal.data();
     Kmers::check(c, fl_results_rows(c, &wr), "fl_results_rows");
+    removed.resize(nr);
+    Kmers::check(c, fl_results_contam(c, nullptr, removed.data(), &contam), "fl_results_contam");
 }
 
 fl_summary ReadSet::finalize(long long total_bases) {

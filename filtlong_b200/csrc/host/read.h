@@ -84,6 +84,10 @@ public:
     std::vector<int32_t> row_s, row_e;
     std::vector<double> row_mean, row_window, row_lscore, row_nmean, row_nwindow, row_final;
     std::vector<uint8_t> row_passed, row_pfinal;
+    // --contam: per read, removed by the contaminant set (all 0 without one), and the removed reads / bases / rows
+    std::vector<uint8_t> removed;
+    fl_contam_counts contam{};
+    bool ranked(size_t row) const { return !removed[row_parent[row]]; }   // the row takes part in the ranking
 
 private:
     fl_ctx *ready_context();                       // the context, with this run's parameters set

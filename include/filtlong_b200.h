@@ -68,6 +68,10 @@ typedef struct fl_params {
      * all >= 33 + trim_q; children are scored on their own quality bytes. 0 = off. A push with trim_q > 0 onto a
      * context whose k-mer set is not empty is FL_EINVAL. */
     int32_t trim_q;
+    /* Not a reference option (--max_contam): a read is removed when more than this percentage of its bases lie in a
+     * 16-mer of the contaminant set (fl_contam_*), compared in double, so a NaN (empty read) never is. Only read when that
+     * set is not empty; a push onto such a context with a value outside [0, 100) is FL_EINVAL. */
+    double max_contam;
 } fl_params;
 
 /* A batch of sequences in the arena layout above. */
@@ -112,7 +116,9 @@ enum { FL_KERNEL_SCORE_PHRED = 0, FL_KERNEL_PROBE_PAINT = 1, FL_KERNEL_KMER_STAT
        /* --trim_q: the quality mask, the two row passes of the mask (with their scan), the gather of the children's
         * quality bytes, and the Phred pass over the children (its kernels also count in FL_KERNEL_SCORE_PHRED) */
        FL_KERNEL_QUAL_MASK = 4, FL_KERNEL_ROW_SCAN = 5, FL_KERNEL_QUAL_GATHER = 6, FL_KERNEL_QUAL_CHILDREN = 7,
-       FL_KERNEL_COUNT = 8 };
+       /* --contam: the probe of the contaminant set, the per-read count and the per-row exclusion */
+       FL_KERNEL_CONTAM = 8,
+       FL_KERNEL_COUNT = 9 };
 int fl_ctx_enable_timing(fl_ctx *ctx, int on);
 int fl_ctx_reset_timing(fl_ctx *ctx);
 int fl_ctx_kernel_time(fl_ctx *ctx, int which, double *total_ms, uint64_t *launches);
@@ -166,6 +172,31 @@ int fl_kmers_release_build_state(fl_ctx *ctx);
  * info[1] = its flavour (bit 2: one word per table group of four 16-mers, bit 3: one word per pair, bit 4: four bits per
  * member), info[2] = log2 of its 64-bit words, info[3] = the position-anchored table is in use. */
 int fl_kmers_probe_info(fl_ctx *ctx, int32_t info[4]);
+
+/* ---- contaminant set (no reference counterpart: --contam) ----------------------------------- */
+/* A second 16-mer set on the same context, built exactly as fl_kmers_add_text / fl_kmers_add_batch build the reference set
+ * with require_multiple_copies == 0 (an assembly: every forward and reverse 16-mer, non-ACGT handling of kmers.cpp:199-219).
+ * It does not decide the scoring mode (that is the reference set's alone). When it is not empty, every push also finds,
+ * per input read, c = 100 * (bases covered by a 16-mer of the set) / length -- the raw mean quality k-mer mode would give
+ * the read against this set -- and removes the read when c > params.max_contam: its rows are not passed, and they take
+ * no part in the statistics, the passed bases or the selection of fl_finalize. The reads' bases are then needed in Phred
+ * mode too (seq2b or ascii; a push without them is FL_EINVAL). Build the set before any read is pushed: an add after
+ * that is FL_EINVAL. About 2.5 GiB of device memory are allocated with the first add. */
+int fl_contam_add_text(fl_ctx *ctx, const char *host_text, uint64_t n_bytes, int format, int is_last_chunk,
+                       uint64_t *n_records, uint64_t *n_bases, uint64_t *bytes_consumed, int *status);
+int fl_contam_add_batch(fl_ctx *ctx, const fl_batch *host_batch);
+int fl_contam_finalize(fl_ctx *ctx, uint64_t *n_kmers_out);
+int fl_contam_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out);
+/* collective, like fl_kmers_broadcast */
+int fl_contam_broadcast(fl_ctx *ctx, int root);
+typedef struct fl_contam_counts {
+    uint64_t reads;    /* input reads removed */
+    int64_t bases;     /* their bases */
+    uint64_t rows;     /* their rows (the reads themselves, or their children) */
+} fl_contam_counts;
+/* Per INPUT READ (length n_reads): percent = c, removed = c > max_contam (0 and 0 when the set is empty); counts of this
+ * context's removed reads. Any pointer may be NULL. */
+int fl_results_contam(fl_ctx *ctx, double *percent, uint8_t *removed, fl_contam_counts *counts);
 
 /* ---- Read: per-read scoring (src/read.cpp:25-144) ------------------------------------------ */
 /* Scores a batch the way one `new Read(...)` per record does (main.cpp:108) and appends the
