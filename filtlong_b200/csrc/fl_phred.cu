@@ -493,6 +493,10 @@ __global__ void k_phred_fill(const int32_t *__restrict__ len, uint32_t n, int ws
 #define PT_THREADS 256
 #define PT_SMEM (256 * 16 * 8)         // one table, 16 lane-private copies = 32 KiB
 #define PS_TILE 512
+// Blocks per SM of k_phred_sum. Three, not the four its shared memory allows: capped at 64 registers the compiler keeps
+// the prefetched uint4 on the stack, and the store that puts it there waits for the load -- every step then pays a full
+// global round trip before it computes. With 85 registers to use (80 used) the load stays in flight during the step.
+#define PS_OCC 3
 
 struct TieInfo {
     unsigned long long any;            // bit e: some table value q ties when added to a sum in [2^e, 2^(e+1))
@@ -555,7 +559,7 @@ __device__ __forceinline__ bool chunk_has(const uint32_t (&cw)[NW], unsigned ch)
     return hit != 0u;
 }
 
-__global__ void __launch_bounds__(PT_THREADS, 4) k_phred_sum(PhredArgs a, TieInfo tie) {
+__global__ void __launch_bounds__(PT_THREADS, PS_OCC) k_phred_sum(PhredArgs a, TieInfo tie) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *tab = reinterpret_cast<double *>(smem_raw);                // q[256][16]
     __shared__ TieInfo s_tie;
@@ -1118,10 +1122,11 @@ int fl_phred_pass(fl_ctx *ctx, const BatchView &b, const PhredOut &o) {
             k_phred_first<<<hb, PH_THREADS, PH_SMEM, st>>>(a);
             ctx->launches++;
         }
-        unsigned blocks = fl_blocks(n * 32, PT_THREADS);
-        const int occ = ctx->phred_occupancy >= 1 && ctx->phred_occupancy <= 6 ? ctx->phred_occupancy : 4;
-        const unsigned cap = (unsigned)ctx->sm_count * (unsigned)occ;
-        if (blocks > cap) blocks = cap;
+        // persistent grids, as many blocks as stay resident: k_phred_sum PS_OCC per SM, k_phred_win 4
+        const bool occ_set = ctx->phred_occupancy >= 1 && ctx->phred_occupancy <= 6;
+        const unsigned want = fl_blocks(n * 32, PT_THREADS);
+        const unsigned sblocks = min(want, (unsigned)ctx->sm_count * (unsigned)(occ_set ? ctx->phred_occupancy : PS_OCC));
+        const unsigned blocks = min(want, (unsigned)ctx->sm_count * (unsigned)(occ_set ? ctx->phred_occupancy : 4));
         {
             // timed as one scoring pass: the sum kernel and the window kernel
             KernelTimer kt(ctx, FL_KERNEL_SCORE_PHRED);
@@ -1132,7 +1137,7 @@ int fl_phred_pass(fl_ctx *ctx, const BatchView &b, const PhredOut &o) {
             // (One fused pass -- a 16-byte {q, a} gather per base feeding both chains, the step one window long -- was
             // built and measured slower: 14 % MORE instructions, because the sum's bookkeeping then runs once per 250 bases
             // instead of once per 512, and 80 registers cost a quarter of the warps; the code is gone.)
-            k_phred_sum<<<blocks, PT_THREADS, PT_SMEM, st>>>(a, ti);
+            k_phred_sum<<<sblocks, PT_THREADS, PT_SMEM, st>>>(a, ti);
             if (ws <= 64) k_phred_win<2><<<blocks, PT_THREADS, PW_SMEM, st>>>(a);
             else if (ws <= 128) k_phred_win<4><<<blocks, PT_THREADS, PW_SMEM, st>>>(a);
             else k_phred_win<8><<<blocks, PT_THREADS, PW_SMEM, st>>>(a);
