@@ -729,9 +729,20 @@ __device__ __forceinline__ void align_raw(const uint32_t (&w)[NW + 1], int pos, 
 #define PW_SHIFT 30                    // filter value of c: A_c >> 30 (A_c < 2^53 / ws, so a window sums to < 2^23)
 #define PW_BAD 0x800000u               // 2^23: filter value of a byte the lattice cannot take
 #define PW_NONE 0xFFFFFFFFu
+#define PW_CHUNK 2048                  // k_phred_win asks L2 for a read's bytes in chunks of this size, one chunk ahead
 #define PW_SMEM (256 * 32 * 4 + 256 * 8 * 8)   // filter table, 32 copies (32 KiB) + grid table, 8 copies (16 KiB)
 // paths a read takes through k_phred_win, counted per read and per base; counter 8 is the exact steps walked
 enum { PW_CAND = 0, PW_FULL = 1, PW_BAD_BYTE = 2, PW_LOW = 3, PW_COUNTERS = 9 };
+
+// asks L2 for bytes [pos, pos + PW_CHUNK) of a read, clamped to its padded extent. Reads start on 64-byte boundaries and
+// own whole 64-byte lines (the clamped word loads rely on the same), so the range is 16-byte aligned, a multiple of 16
+// long, and never leaves the arena. The filter pass has one step of loads in flight per warp; with the next chunk
+// already on its way to L2 those loads wait for L2, not for HBM.
+__device__ __forceinline__ void prefetch_chunk(const uint8_t *q, int pos, int padded) {
+    if (pos >= padded) return;
+    const int end = pos + PW_CHUNK < padded ? pos + PW_CHUNK : padded;
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(q + pos), "r"((uint32_t)(end - pos)) : "memory");
+}
 
 // inclusive warp scan; the shuffle's own predicate says whether the source lane exists (no lane tests)
 __device__ __forceinline__ uint32_t warp_incl_scan_u32(uint32_t v) {
@@ -902,8 +913,10 @@ __global__ void __launch_bounds__(PT_THREADS, 4) k_phred_win(PhredArgs a) {
         const uint32_t r = a.order[it];
         const int L = a.len[r];
         if (L <= ws) continue;                                         // finished by k_phred_first
-        const uint32_t *q32 = reinterpret_cast<const uint32_t *>(a.qual + a.off[r]);
-        const int maxword = (((L + 63) & ~63) >> 2) - 1;
+        const uint8_t *q = a.qual + a.off[r];
+        const uint32_t *q32 = reinterpret_cast<const uint32_t *>(q);
+        const int padded = (L + 63) & ~63;
+        const int maxword = (padded >> 2) - 1;
         const int nsteps = (L - 1) / ws;
         const double W0 = a.it_b[r];                                   // fl(sum of the first window / ws), read.cpp:223
         bool reject = !(W0 >= thr && W0 < 1.0);
@@ -926,6 +939,11 @@ __global__ void __launch_bounds__(PT_THREADS, 4) k_phred_win(PhredArgs a) {
             uint32_t W = S0f;                                          // sum of the window ending at base j - 1
             reject = W >= PW_BAD;
             uint32_t pre[NW + 1];
+            if (lane == 0) {
+                prefetch_chunk(q, 0, padded);
+                prefetch_chunk(q, PW_CHUNK, padded);
+            }
+            int pf = 2 * PW_CHUNK;                                     // the next chunk to ask L2 for
             load_raw<NW>(q32, ws + lpos, maxword, pre);
             int j = ws, t = 0;
             // one step: bases [j, j + ws) (fewer in the last one). A byte that enters the window in this step is
@@ -933,6 +951,10 @@ __global__ void __launch_bounds__(PT_THREADS, 4) k_phred_win(PhredArgs a) {
 #define PW_STEP(WAS, NOW)                                                                                     \
             {                                                                                                 \
                 uint32_t cw[NW];                                                                              \
+                if (j + ws > pf - PW_CHUNK) {       /* the step reaches the chunk before pf: ask for pf's */  \
+                    if (lane == 0) prefetch_chunk(q, pf, padded);                                             \
+                    pf += PW_CHUNK;                                                                           \
+                }                                                                                             \
                 align_raw<NW>(pre, j + lpos, cw);                                                             \
                 if (j + ws < L) load_raw<NW>(q32, j + ws + lpos, maxword, pre);                               \
                 const int n = L - j;                                                                          \

@@ -9,6 +9,7 @@
 //   MODE 2  the same ring, filled by every lane with 16-byte cp.async
 // DEEP: the warp holds the next read's descriptor while it walks this one, the ring is refilled across the read
 // boundary, and short reads are claimed eight per atomicAdd. Without it a read starts cold.
+// k_chunked (below): the same walks cut into chunks, with a bulk L2 prefetch ahead, and both walks in one pass.
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -227,6 +228,106 @@ __global__ void __launch_bounds__(THREADS) k_probe(Args a) {
             feed.end_read(L, a.qual, lane);
         }
     }
+}
+
+// Chunked walks with a bulk L2 prefetch. The read is cut into chunks of CH bytes; on entering chunk c lane 0 issues
+// cp.async.bulk.prefetch.L2 for chunk c + D (chunks 0 .. D-1 at the read's start), clamped to the read's padded extent
+// (offsets are 64-byte aligned, extents whole 64-byte lines, so every prefetch is 16-byte aligned and a multiple of 16).
+// The loads themselves stay one step ahead in registers, as in MODE 0. D = 0: no bulk prefetch.
+//   KIND 0  k_phred_sum's walk, KIND 1  k_phred_win's walk, each on its own
+//   KIND 2  both over the same chunk: the sum's 512-byte steps that start in it, then the window steps that end in it
+__device__ __forceinline__ void prefetch_chunk(const uint8_t *q, int pos, int bytes, int padded) {
+    if (pos >= padded) return;
+    const int end = pos + bytes < padded ? pos + bytes : padded;
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(q + pos), "r"((uint32_t)(end - pos)) : "memory");
+}
+
+template <int KIND, int CH, int D>
+__global__ void __launch_bounds__(THREADS) k_chunked(Args a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const unsigned lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < a.table_bytes / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem_raw)[i] = 0u;
+    __syncthreads();
+    const int skip = KIND == 0 ? H : WS;
+    for (;;) {
+        unsigned long long it = 0;
+        if (lane == 0) it = atomicAdd(a.work, 1ull);
+        it = __shfl_sync(FULL, it, 0);
+        if (it >= a.n) break;
+        const uint32_t r = a.order[it];
+        const int L = a.len[r];
+        if (L <= skip) continue;
+        const uint8_t *q = a.qual + a.off[r];
+        const int padded = (L + 63) & ~63;
+        const uint4 *qv = reinterpret_cast<const uint4 *>(q);
+        const uint32_t *q32 = reinterpret_cast<const uint32_t *>(q);
+        const int maxword = (padded >> 2) - 1;
+        uint32_t x = 0;
+        uint4 spre = make_uint4(0u, 0u, 0u, 0u);
+        uint32_t wpre[NW + 1];
+        if (KIND != 1 && H + 16 * (int)lane < L) spre = __ldg(qv + ((H >> 4) + (int)lane));
+        if (KIND != 0) {
+#pragma unroll
+            for (int i = 0; i <= NW; ++i) wpre[i] = __ldg(q32 + min(((K * (int)lane) >> 2) + i, maxword));
+        }
+        if (D > 0 && lane == 0)
+            for (int c = 0; c < D; ++c) prefetch_chunk(q, c * CH, CH, padded);
+        int js = H, jw = 0;                  // next sum step, next window step
+        for (int c0 = 0; c0 < L; c0 += CH) {
+            const int cend = c0 + CH < L ? c0 + CH : L;
+            if (D > 0 && lane == 0) prefetch_chunk(q, c0 + D * CH, CH, padded);
+            if (KIND != 1) {
+                for (; js < cend; js += TILE) {
+                    x ^= spre.x ^ spre.y ^ spre.z ^ spre.w;
+                    const int pn = js + TILE + 16 * (int)lane;
+                    if (pn < L) spre = __ldg(qv + (pn >> 4));
+                }
+            }
+            if (KIND != 0) {
+                for (; jw < L && min(jw + WS, L) <= cend; jw += WS) {
+                    x ^= wpre[0] ^ wpre[1] ^ wpre[2];
+                    if (jw + WS < L) {
+#pragma unroll
+                        for (int i = 0; i <= NW; ++i) wpre[i] = __ldg(q32 + min(((jw + WS + K * (int)lane) >> 2) + i, maxword));
+                    }
+                }
+            }
+        }
+        x = __reduce_xor_sync(FULL, x);
+        if (lane == 0) a.out[r] = x;
+    }
+}
+
+template <int KIND, int CH, int D>
+static int launch_chunked(const Args &a, int sms, int occ, cudaStream_t st) {
+    auto k = k_chunked<KIND, CH, D>;
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, a.table_bytes);
+    if (e != cudaSuccess) return (int)e;
+    int resident = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, k, THREADS, a.table_bytes);
+    if (e != cudaSuccess) return (int)e;
+    if (resident < 1) return -2;
+    if (occ > resident) occ = resident;
+    k<<<sms * occ, THREADS, a.table_bytes, st>>>(a);
+    return -(100 + occ);
+}
+
+// Runs one chunked probe launch with table_bytes of dynamic shared memory; returns as probe_launch does.
+extern "C" int chunked_launch(int kind, int ch, int depth, int table_bytes, int occ, const void *qual, const void *off,
+                              const void *len, const void *order, uint32_t n, void *work, void *out, int sms, void *stream) {
+    Args a;
+    a.qual = (const uint8_t *)qual; a.off = (const unsigned long long *)off; a.len = (const int32_t *)len;
+    a.order = (const uint32_t *)order; a.n = n; a.work = (unsigned long long *)work; a.out = (uint32_t *)out;
+    a.table_bytes = table_bytes;
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaError_t e = cudaMemsetAsync(work, 0, 8, st);
+    if (e != cudaSuccess) return (int)e;
+#define CCASE(KIND_, CH_, D_) \
+    if (kind == KIND_ && ch == CH_ && depth == D_) return launch_chunked<KIND_, CH_, D_>(a, sms, occ, st);
+#define CDS(KIND_, CH_) CCASE(KIND_, CH_, 0) CCASE(KIND_, CH_, 1) CCASE(KIND_, CH_, 2)
+#define CKINDS(KIND_) CDS(KIND_, 2048) CDS(KIND_, 4096) CDS(KIND_, 8192)
+    CKINDS(0) CKINDS(1) CKINDS(2)
+    return -1;
 }
 
 template <int KIND, int MODE, int D, bool DEEP>

@@ -9,7 +9,12 @@ Part 2, load-only probes (tools/phred_loads.cu, compiled here with the library's
 never linked into the library): the same claim loop, addresses and shared-memory footprint as each kernel, the per-base
 work replaced by an XOR. Variants: loads one step ahead in registers; a per-warp shared-memory ring of 2, 4 or 8 tiles
 filled by cp.async.bulk or by per-lane cp.async; reads taken longest first or in arena order; the next read claimed
-and prefetched while this one is walked, or not. Times are CUDA events over --launches launches.
+and prefetched while this one is walked, or not. Then the chunked walks, with the shared-memory footprint of a
+one-pass kernel that would hold both chains' tables (72 KiB, three blocks per SM): each read cut into chunks of 2, 4 or
+8 KiB, lane 0 asking L2 for the chunk D = 1 or 2 ahead with cp.async.bulk.prefetch.L2 (D = 0: no prefetch), the loads
+one step ahead in registers; k_phred_sum's walk, k_phred_win's walk, and one pass doing both per chunk (the sum's
+512-byte steps that start in the chunk, then the window steps that end in it). Times are CUDA events over --launches
+launches.
 
     python tools/phred_loads.py [--scale 1.0] [--steps 3] [--launches 5] [--skip-library] [--skip-probes]
 
@@ -102,6 +107,8 @@ def build_probes(tmp):
     lib = ctypes.CDLL(so)
     lib.probe_launch.restype = ctypes.c_int
     lib.probe_launch.argtypes = [ctypes.c_int] * 5 + [ctypes.c_void_p] * 4 + [ctypes.c_uint32] + [ctypes.c_void_p] * 2 + [ctypes.c_int, ctypes.c_void_p]
+    lib.chunked_launch.restype = ctypes.c_int
+    lib.chunked_launch.argtypes = lib.probe_launch.argtypes
     return lib
 
 
@@ -150,8 +157,42 @@ def probe_part(torch, dev, stream, args):
                     ms = e0.elapsed_time(e1) / args.launches
                     cells.append("%7.2f ms (%6.0f GB/s) [%d]" % (ms, w["padded"] / ms / 1e6, occ))
                 print("%-20s %-34s %28s %28s" % (name, label, cells[0], cells[1]))
+            chunked_part(torch, dev, stream, args, lib, sms, name, w, d_qual, t_off, t_len, longest, work, out)
             del d_qual, t_len, t_off, longest, arena, out
             torch.cuda.empty_cache()
+
+
+# Dynamic shared memory of the one-pass kernel's tables: the sum's (32 KiB), the window filter's (32 KiB) and the
+# window's grid table in 4 copies (8 KiB). Three blocks of 256 threads fit an SM.
+CHAIN_SMEM = 73728
+
+
+def chunked_part(torch, dev, stream, args, lib, sms, name, w, d_qual, t_off, t_len, order, work, out):
+    """Chunked walks, register loads plus a bulk L2 prefetch D chunks ahead (D = 0: none), longest first, with the
+    one-pass kernel's shared-memory footprint and three blocks per SM."""
+    print("chunked walks, %d B of tables, ms per launch (GB/s of arena bytes) [blocks per SM that ran]:" % CHAIN_SMEM)
+    print("%-20s %6s %2s %28s %28s %28s" % ("lengths", "chunk", "D", "k_phred_sum's walk", "k_phred_win's walk", "one pass, both"))
+    for ch in (2048, 4096, 8192):
+        for depth in (0, 1, 2):
+            cells = []
+            for kind in (0, 1, 2):
+                def launch():
+                    rc = lib.chunked_launch(kind, ch, depth, CHAIN_SMEM, 3, d_qual.data_ptr(), t_off.data_ptr(), t_len.data_ptr(),
+                                            order.data_ptr(), w["n"], work.data_ptr(), out.data_ptr(), sms, stream.cuda_stream)
+                    if rc > -100:
+                        raise RuntimeError("chunked probe %d/%d/%d: error %d" % (kind, ch, depth, rc))
+                    return -rc - 100
+                occ = launch()
+                torch.cuda.synchronize(dev)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                for _ in range(args.launches):
+                    launch()
+                e1.record(stream)
+                torch.cuda.synchronize(dev)
+                ms = e0.elapsed_time(e1) / args.launches
+                cells.append("%7.2f ms (%6.0f GB/s) [%d]" % (ms, w["padded"] / ms / 1e6, occ))
+            print("%-20s %6d %2d %28s %28s %28s" % (name, ch, depth, cells[0], cells[1], cells[2]))
 
 
 def main():
