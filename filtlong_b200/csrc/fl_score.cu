@@ -450,7 +450,10 @@ __global__ void __launch_bounds__(256) k_kmer_scan(ScanArgs a) {
 // tests/models/kmer_window_model.c is the scalar model of exactly this procedure (fuzzed against the reference
 // recurrence: tests/test_kmer_window_model.py); the kernel below is its transcription, 32 words per iteration.
 // ---------------------------------------------------------------------------------------------
-#define KW_MAX_EDGES 16
+// one edge for every binade from rq's own up to 2^1: at most 33 for an int window size (rq >= 2^-31). Dropping one lets the
+// chain cross that edge as if it were inside a binade: at ws >= 2^15 (more than 16 binades) the window quality of a row
+// hovering at half coverage came out one ulp off (tests/test_gpu_kmer_masks.py).
+#define KW_MAX_EDGES 34
 
 struct KwConsts {
     double rq;

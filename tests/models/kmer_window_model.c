@@ -33,12 +33,16 @@
 #include <stdint.h>
 #include <string.h>
 
+/* one edge for every binade from rq's own up to 2^1: at most 33 for a window size below 2^31 (rq >= 2^-31). Dropping
+ * one would let the chain cross that edge as if it were inside a binade (a window quality one ulp off at ws >= 2^15). */
+#define KW_MAX_EDGES 34
+
 typedef struct {
     double rq;
     int e_rq;             /* rq in [2^e_rq, 2^(e_rq+1)) */
     uint64_t mant_rq;     /* 53-bit significand of rq */
     int n_edges;          /* count intervals around the binade edges 2^e / rq (two levels of margin) */
-    int elo[16], ehi[16];
+    int elo[KW_MAX_EDGES], ehi[KW_MAX_EDGES];
 } chain_consts;
 
 typedef struct {
@@ -59,7 +63,7 @@ void kw_consts(chain_consts *k, int ws) {
     k->e_rq = (int)((b >> 52) & 0x7FF) - 1023;
     k->mant_rq = ((uint64_t)b & ((1ull << 52) - 1ull)) | (1ull << 52);
     k->n_edges = 0;
-    for (int e = k->e_rq; e <= 1 && k->n_edges < 16; ++e) {           /* edges 2^e for every binade a count 0..ws can reach */
+    for (int e = k->e_rq; e <= 1 && k->n_edges < KW_MAX_EDGES; ++e) {           /* edges 2^e for every binade a count 0..ws can reach */
         const double x = ldexp(1.0, e) * (double)ws;
         if (x > (double)ws + 3.0) break;
         k->elo[k->n_edges] = (int)floor(x) - 2;

@@ -13,7 +13,8 @@ from tests import parity, util
 pytestmark = pytest.mark.gpu
 
 
-def run_both(reads, opts, assembly=None, short=None):
+def run_both(reads, opts, assembly=None, short=None, cap=4096):
+    """the oracle and the device on the same reads; `cap` bounds the oracle's bad ranges and children per read"""
     p, op = api.make_params(**opts), orc.make_params(**opts)
     ok = None
     if assembly or short:
@@ -22,7 +23,7 @@ def run_both(reads, opts, assembly=None, short=None):
             ok.add_assembly(assembly)
         for f in short or []:
             ok.add_short_reads(f)
-    sc = orc.finalize(orc.score(reads, op, ok), op)
+    sc = orc.finalize(orc.score(reads, op, ok, cap=cap), op)
     ctx, summ = api.score_and_filter(reads, p, assembly=assembly, short_reads=short)
     return ctx, summ, sc, ok
 

@@ -123,3 +123,46 @@ def test_realistic_masks_are_nearly_event_free(model):
         a = model.kmer_window_model(m.ctypes.data, 0, len(bits), 250, None, C.byref(ns))
         assert a.hex() == model.kmer_window_reference(m.ctypes.data, 0, len(bits), 250).hex()
         assert ns.value / (len(bits) / 32) <= bound, (err, ns.value)
+
+
+def _family(rng, fam, n, ws):
+    from tests import kmer_masks as km
+    if fam == "opened":                                  # the model kinds made paintable: every 1-run >= 16 bases
+        return km.opening(make_mask(rng, int(rng.integers(0, 7)), n))
+    if fam == "rising":                                  # sparse or empty first window, then gaps shrinking to full coverage
+        return km.rising(rng, n, ws, int(rng.integers(0, 2)))
+    return make_mask(rng, int(rng.integers(0, 7)), n)
+
+
+@pytest.mark.parametrize("ws", list(range(1, 16)) + [32767, 32768, 32769, 65536, 100000])
+def test_model_at_tiny_and_huge_window_sizes(model, ws):
+    """ws 1..15 (rq = 1, 1/2, 1/3 ...: almost no grid below the count's binade) and ws >= 2^15 (more than 16 binade
+    edges, the most a window size below 2^31 needs is 33), on the model's mask kinds, their openings and rising rows."""
+    rng = np.random.default_rng(ws)
+    slow = 0
+    for it in range(45 if ws < 16 else 6):
+        fam = ("raw", "opened", "rising")[it % 3]
+        n = int(rng.integers(ws + 1, ws * (20 if ws < 16 else 3) + 3000))
+        m = pack(_family(rng, fam, n, ws))
+        for S, E in ((0, n), (int(rng.integers(0, n // 2)), int(rng.integers(n // 2, n + 1)))):
+            if E <= S:
+                continue
+            ns = C.c_longlong()
+            a = model.kmer_window_model(m.ctypes.data, S, E, ws, None, C.byref(ns))
+            b = model.kmer_window_reference(m.ctypes.data, S, E, ws)
+            assert struct.pack("<d", a) == struct.pack("<d", b), (it, fam, n, ws, S, E, a.hex(), b.hex())
+            slow += ns.value
+    assert slow > 0
+
+
+def test_a_row_hovering_at_half_with_more_than_16_edges(model):
+    """ws = 100000 has 18 binade edges; a row whose count hovers around ws / 2 after a long climb needs the edge at
+    0.5 (the model once kept only 16 edges and came out one ulp off here)."""
+    from tests import kmer_masks as km
+    rng = np.random.default_rng(3)
+    ws = 100000
+    for _ in range(4):
+        bits = km.hover(rng, 4 * ws, ws, ws // 2, False)
+        m = pack(bits)
+        a = model.kmer_window_model(m.ctypes.data, 0, len(bits), ws, None, None)
+        assert a.hex() == model.kmer_window_reference(m.ctypes.data, 0, len(bits), ws).hex()
