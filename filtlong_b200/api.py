@@ -189,6 +189,32 @@ class Context:
         self._ck(self.L.fl_contam_export(self.h, capi.ptr(out), n, C.byref(got)), "fl_contam_export")
         return out[:n]
 
+    def contam_configure(self, k, max_kmers=0):
+        """fl_contam_configure: k-mers of k = 16..32 bases, a set of k > 16 sized for max_kmers canonical k-mers."""
+        self._ck(self.L.fl_contam_configure(self.h, int(k), int(max_kmers)), "fl_contam_configure")
+
+    def contam_export64(self):
+        """the canonical members of a set of k > 16, sorted"""
+        n = C.c_uint64()
+        self._ck(self.L.fl_contam_export64(self.h, None, 0, C.byref(n)), "fl_contam_export64")
+        out = np.zeros(max(n.value, 1), dtype=np.uint64)
+        got = C.c_uint64()
+        self._ck(self.L.fl_contam_export64(self.h, capi.ptr(out), n.value, C.byref(got)), "fl_contam_export64")
+        return np.sort(out[:n.value])
+
+    def contam_contains64(self, fwd_kmers):
+        """per forward k-mer (2-bit codes, first base high): in a set of k > 16 on either strand"""
+        q = np.ascontiguousarray(fwd_kmers, dtype=np.uint64)
+        out = np.zeros(max(len(q), 1), dtype=np.uint8)
+        self._ck(self.L.fl_contam_contains64(self.h, capi.ptr(q), len(q), capi.ptr(out)), "fl_contam_contains64")
+        return out[:len(q)].astype(bool)
+
+    def contam_probe_lengths(self, n_bins=16):
+        """(members by sectors read per look-up, buckets by sectors an absent k-mer's look-up reads); last bin = or more"""
+        h = np.zeros(2 * n_bins, dtype=np.uint64)
+        self._ck(self.L.fl_contam_probe_lengths(self.h, capi.ptr(h), n_bins), "fl_contam_probe_lengths")
+        return h[:n_bins], h[n_bins:]
+
     def contam_broadcast(self, root=0):
         self._ck(self.L.fl_contam_broadcast(self.h, root), "fl_contam_broadcast")
 

@@ -158,6 +158,10 @@ SYMBOLS = [
     ("fl_contam_finalize", C.c_int, [_P, C.POINTER(C.c_uint64)]),
     ("fl_contam_export", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("fl_contam_broadcast", C.c_int, [_P, C.c_int]),
+    ("fl_contam_configure", C.c_int, [_P, C.c_int, C.c_uint64]),
+    ("fl_contam_export64", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("fl_contam_contains64", C.c_int, [_P, _P, C.c_uint32, _P]),
+    ("fl_contam_probe_lengths", C.c_int, [_P, _P, C.c_int]),
     ("fl_results_contam", C.c_int, [_P, _P, _P, C.POINTER(ContamCounts)]),
     ("fl_reads_push", C.c_int, [_P, C.POINTER(Batch)]),
     ("fl_reads_push_text", C.c_int, [_P, _P, C.c_uint64, C.c_int, C.c_int, C.POINTER(TextRecords), C.POINTER(C.c_uint64),

@@ -130,6 +130,13 @@ int fl_comm_allreduce_u64(fl_ctx *ctx, unsigned long long *buf, size_t n) {
     return FL_OK;
 }
 
+int fl_comm_broadcast_bytes(fl_ctx *ctx, void *buf, size_t bytes, int root) {
+    if (!ctx->comm) return FL_OK;
+    FL_NCCL(ctx, nccl().Broadcast(buf, buf, bytes, ncclUint8, root, static_cast<ncclComm_t>(ctx->comm), ctx->stream));
+    ctx->collectives++;
+    return FL_OK;
+}
+
 extern "C" int fl_comm_allreduce_i64_host(fl_ctx *ctx, int64_t *inout, int n) {
     FL_ENTER(ctx);
     if (!inout || n < 0 || (size_t)n * 8 > 256) return FL_EINVAL;
@@ -147,6 +154,7 @@ extern "C" int fl_comm_allreduce_i64_host(fl_ctx *ctx, int64_t *inout, int n) {
 // over NVLink; each rank then derives its own probe tables from it (fl_kmers_recount).
 static int broadcast_set(fl_ctx *ctx, KmerSet &s, int root, const char *entry) {
     if (root < 0 || root >= ctx->comm_nranks) { ctx->set_error(std::string(entry) + ": bad root"); return FL_EINVAL; }
+    if (s.k > 16) return fl_ck_broadcast(ctx, s, root);     // every rank configured the same k and size (fl_contam_configure)
     if (ctx->comm_rank == root && (s.stale || (&s == &ctx->ref && ctx->multi_pending))) FL_TRY(fl_kmers_recount(ctx, s));
     FL_TRY(fl_kmers_ensure_bitmap(ctx, s));
     if (!ctx->comm) return FL_OK;
@@ -162,8 +170,36 @@ extern "C" int fl_kmers_broadcast(fl_ctx *ctx, int root) {
     return broadcast_set(ctx, ctx->ref, root, "fl_kmers_broadcast");
 }
 
+// A contaminant set of k > 16 goes as its table's bytes, so every rank must hold one of the same k and size. Two small
+// collectives (the root's k and bucket count out, then the sum of the ranks' disagreements) let every rank see a mismatch
+// and return FL_EINVAL together, instead of issuing broadcasts of different sizes.
+static int check_same_contam(fl_ctx *ctx, int root) {
+    if (!ctx->comm) return FL_OK;
+    if (root < 0 || root >= ctx->comm_nranks) { ctx->set_error("fl_contam_broadcast: bad root"); return FL_EINVAL; }
+    const KmerSet &s = ctx->contam;
+    unsigned long long *d = ctx->d_scalars + 48, *h = ctx->h_scalars + 48;
+    h[0] = (unsigned long long)s.k;
+    h[1] = s.n_buckets;
+    FL_CUDA(ctx, cudaMemcpyAsync(d, h, 2 * sizeof(unsigned long long), cudaMemcpyHostToDevice, ctx->stream));
+    FL_TRY(fl_comm_broadcast_bytes(ctx, d, 2 * sizeof(unsigned long long), root));
+    FL_CUDA(ctx, cudaMemcpyAsync(h + 2, d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+    FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    h[4] = (h[2] != (unsigned long long)s.k || h[3] != s.n_buckets) ? 1ull : 0ull;
+    FL_CUDA(ctx, cudaMemcpyAsync(d + 4, h + 4, sizeof(unsigned long long), cudaMemcpyHostToDevice, ctx->stream));
+    FL_TRY(fl_comm_allreduce_u64(ctx, d + 4, 1));
+    FL_CUDA(ctx, cudaMemcpyAsync(h + 5, d + 4, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+    FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (h[5]) {
+        ctx->set_error("fl_contam_broadcast: the ranks' contaminant sets differ in k or table size (fl_contam_configure every "
+                       "rank with the same k and max_kmers)");
+        return FL_EINVAL;
+    }
+    return FL_OK;
+}
+
 extern "C" int fl_contam_broadcast(fl_ctx *ctx, int root) {
     FL_ENTER(ctx);
+    FL_TRY(check_same_contam(ctx, root));
     return broadcast_set(ctx, ctx->contam, root, "fl_contam_broadcast");
 }
 

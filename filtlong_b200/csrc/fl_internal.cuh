@@ -131,11 +131,19 @@ struct KmerSet {
     bool use_filter = false;
     uint32_t *anchor = nullptr;          // position-anchored membership table (2 GiB), see fl_anchor_slot
     bool use_anchor = false;
+    bool added = false;                  // something was added (fl_contam_configure comes first)
+    // k = 16: the bitmap and tables above. k = 17..32 (the contaminant set only, fl_contam_configure): a hash set of
+    // canonical k-mers, 4 slots per bucket, then two counters: distinct members, palindromes (fl_contam_k.cu)
+    int k = 16;
+    unsigned long long *table = nullptr;
+    uint64_t n_buckets = 0;
+    uint64_t limit = 0;                  // the most members the table may hold (its load limit)
     void release() {
         if (bitmap) cudaFree(bitmap);
         if (filter) cudaFree(filter);
         if (anchor) cudaFree(anchor);
-        bitmap = nullptr; filter = nullptr; anchor = nullptr;
+        if (table) cudaFree(table);
+        bitmap = nullptr; filter = nullptr; anchor = nullptr; table = nullptr;
     }
 };
 
@@ -316,6 +324,13 @@ int fl_sets_ready(fl_ctx *ctx);
 // FL_EINVAL (with a message) when the contaminant set is added to after reads were pushed
 int fl_contam_check_order(fl_ctx *ctx);
 
+// ---- implemented in fl_contam_k.cu (a set with k > 16) ----
+int fl_ck_add_view(fl_ctx *ctx, KmerSet &s, const BatchView &b);
+int fl_ck_recount(fl_ctx *ctx, KmerSet &s);
+// the same mask as fl_probe_paint: 1 bit per padded base of b, the base is covered by a k-mer of s
+int fl_ck_paint(fl_ctx *ctx, const KmerSet &s, const BatchView &b, uint32_t *mask, int timer);
+int fl_ck_broadcast(fl_ctx *ctx, KmerSet &s, int root);
+
 // ---- implemented in fl_score.cu ----
 // defer = the caller will call fl_score_complete() later (fl_reads_push: after the NEXT batch's copy is under way), so
 // that the one host round trip of --trim / --split (how many rows did this batch make?) does not stall the copy pipeline
@@ -353,6 +368,7 @@ int fl_score_qual_rows(fl_ctx *ctx, const BatchView &b, size_t n_rows_batch);
 // ---- implemented in fl_comm.cu (no-ops / plain copies on a context without a communicator) ----
 int fl_comm_allgather(fl_ctx *ctx, const void *send, void *recv, size_t bytes_per_rank);
 int fl_comm_allreduce_u64(fl_ctx *ctx, unsigned long long *buf, size_t n);
+int fl_comm_broadcast_bytes(fl_ctx *ctx, void *buf, size_t bytes, int root);
 
 // ---- implemented in fl_select.cu ----
 int fl_norm_select_free(fl_ctx *ctx);

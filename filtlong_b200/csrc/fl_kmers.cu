@@ -286,6 +286,8 @@ static int ensure_multi_state(fl_ctx *ctx) {
 
 int fl_kmers_add_view(fl_ctx *ctx, KmerSet &s, const BatchView &b, int multi) {
     if (b.n == 0) return FL_OK;
+    s.added = true;
+    if (s.k > 16) return fl_ck_add_view(ctx, s, b);
     if (!b.seq2b) { ctx->set_error("fl_kmers_add_batch: seq2b is required"); return FL_EINVAL; }
     FL_TRY(fl_kmers_ensure_bitmap(ctx, s));
     if (multi) FL_TRY(ensure_multi_state(ctx));
@@ -330,6 +332,7 @@ int fl_kmers_add_view(fl_ctx *ctx, KmerSet &s, const BatchView &b, int multi) {
 }
 
 int fl_kmers_recount(fl_ctx *ctx, KmerSet &s) {
+    if (s.k > 16) return fl_ck_recount(ctx, s);
     if (!s.bitmap) { s.n = 0; s.stale = false; return FL_OK; }
     if (ctx->multi_pending && &s == &ctx->ref) {
         unsigned blocks = (unsigned)ctx->sm_count * 16;
@@ -488,6 +491,7 @@ extern "C" int fl_contam_finalize(fl_ctx *ctx, uint64_t *n_kmers_out) {
 
 extern "C" int fl_contam_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out) {
     FL_ENTER(ctx);
+    if (ctx->contam.k > 16) { ctx->set_error("fl_contam_export: the contaminant set holds longer k-mers (fl_contam_export64)"); return FL_EINVAL; }
     FL_TRY(fl_contam_finalize(ctx, nullptr));
     return export_set(ctx, ctx->contam, out, cap, n_out);
 }

@@ -810,7 +810,7 @@ __global__ void k_identity_rows(uint32_t n, const int32_t *__restrict__ len, uin
     w_end[i] = len[i];
 }
 
-// --contam, per read: the percentage of its bases covered by a contaminant 16-mer, in the expression k_kmer_window
+// --contam, per read: the percentage of its bases covered by a contaminant k-mer, in the expression k_kmer_window
 // evaluates for a read's mean in k-mer mode (read.cpp:208-213: 0 below 16 bases, NaN for an empty read), and whether it
 // is above max_contam (a NaN never is). One warp per read over its mask words.
 __global__ void __launch_bounds__(256) k_contam_reads(const uint32_t *__restrict__ mask, const uint64_t *__restrict__ off,
@@ -1116,7 +1116,8 @@ static int contam_reads(fl_ctx *ctx, const BatchView &b) {
     FL_CUDA(ctx, ctx->r_contam.reserve(rb + n, rb, st));
     FL_CUDA(ctx, ctx->r_removed.reserve(rb + n, rb, st));
     FL_CUDA(ctx, ctx->sc_cmask.reserve((size_t)(b.padded_bases >> 5) + 1, 0, st));
-    FL_TRY(fl_probe_paint(ctx, ctx->contam, b, ctx->sc_cmask.p, FL_KERNEL_CONTAM));
+    if (ctx->contam.k > 16) FL_TRY(fl_ck_paint(ctx, ctx->contam, b, ctx->sc_cmask.p, FL_KERNEL_CONTAM));
+    else FL_TRY(fl_probe_paint(ctx, ctx->contam, b, ctx->sc_cmask.p, FL_KERNEL_CONTAM));
     {
         KernelTimer kt(ctx, FL_KERNEL_CONTAM);
         k_contam_reads<<<scan_blocks_of(ctx, n), 256, 0, st>>>(ctx->sc_cmask.p, b.off, b.len, b.n, ctx->p.max_contam,

@@ -79,6 +79,15 @@ int read_trim_q(const std::string &value) {
     return std::stoi(value.substr(digits));
 }
 
+// --contam_k (not a reference option): digits only, 16 to 32
+int read_contam_k(const std::string &value) {
+    const size_t digits = value.find_first_not_of('0');
+    const bool ok = !value.empty() && value.find_first_not_of("0123456789") == std::string::npos && digits != std::string::npos &&
+                    value.size() - digits <= 2 && std::stoi(value.substr(digits)) >= 16 && std::stoi(value.substr(digits)) <= 32;
+    if (!ok) throw ParseError("Error: the value for --contam_k must be an integer from 16 to 32");
+    return std::stoi(value.substr(digits));
+}
+
 long long read_plain_ll(const std::string &name, const std::string &value) {         // args.h default reader
     std::istringstream ss(value);
     long long v = 0;
@@ -109,8 +118,9 @@ const Opt kOpts[] = {
     {0, "length_weight", true, "float", "weight given to the length score (default: 1)"},
     {0, "mean_q_weight", true, "float", "weight given to the mean quality score (default: 1)"},
     {0, "window_q_weight", true, "float", "weight given to the window quality score (default: 1)"},
-    {0, "contam", true, "file", "remove reads that come from these sequences (FASTA or FASTQ, may be gzipped), judged by their 16-mers (not a reference option)"},
-    {0, "max_contam", true, "float", "remove a read when more than this percentage of its bases lie in a 16-mer of --contam (default: 50; not a reference option)"},
+    {0, "contam", true, "file", "remove reads that come from these sequences (FASTA or FASTQ, may be gzipped), judged by their k-mers (16-mers unless --contam_k; not a reference option)"},
+    {0, "max_contam", true, "float", "remove a read when more than this percentage of its bases lie in a k-mer of --contam (default: 50; not a reference option)"},
+    {0, "contam_k", true, "int", "judge reads by the contaminant's k-mers of this length, 16 to 32 (default: 16; longer k-mers suit a large contaminant such as a host genome; not a reference option)"},
     {0, "trim", false, "trim", "trim non-k-mer-matching bases from start/end of reads"},
     {0, "split", true, "split", "split reads at this many (or more) consecutive non-k-mer-matching bases (unit suffixes: k, kb, m, mb, g, gb)"},
     {0, "trim_q", true, "int", "without a reference, --trim / --split on Phred scores: a base is good if it lies in 16 consecutive bases of at least this quality (1 to 93; not a reference option)"},
@@ -133,9 +143,9 @@ void print_help(const char *prog) {
         {"output thresholds:", 0, 5},
         {"external references (if provided, read quality will be determined using these instead of from the Phred scores):", 6, 8},
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
-        {"contaminant removal:", 12, 13},
-        {"read manipulation:", 14, 16},
-        {"other:", 17, 23},
+        {"contaminant removal:", 12, 14},
+        {"read manipulation:", 15, 17},
+        {"other:", 18, 24},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -177,6 +187,7 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "window_q_weight") window_q_weight = read_double(nm, v);
         else if (ln == "contam") { contam = v; contam_set = true; }
         else if (ln == "max_contam") { max_contam = read_double(nm, v); max_contam_set = true; }
+        else if (ln == "contam_k") { contam_k = read_contam_k(v); contam_k_set = true; }
         else if (ln == "trim") trim = true;
         else if (ln == "split") { split = read_int_suffix(nm, v); split_set = true; }
         else if (ln == "trim_q") trim_q = read_trim_q(v);
@@ -256,6 +267,7 @@ Arguments::Arguments(int argc, char **argv) {
     if (trim && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --trim");
     if (split_set && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --split");
     if (max_contam_set && !contam_set) FAIL("Error: --max_contam needs --contam");
+    if (contam_k_set && !contam_set) FAIL("Error: --contam_k needs --contam");
     if (contam_set && !(max_contam >= 0.0 && max_contam < 100.0))
         FAIL("Error: the value for --max_contam must be at least 0 and less than 100");
     if (!reads_exist(input_reads)) FAIL("Error: cannot find file: " + input_reads);

@@ -45,6 +45,8 @@ public:
     std::string contam;
     bool max_contam_set = false;
     double max_contam = 50.0;
+    bool contam_k_set = false;
+    int contam_k = 16;            // the length of the contaminant k-mers (16 to 32)
 
     int window_size = 250;
     bool verbose = false;

@@ -221,7 +221,7 @@ ChunkPush bam_push(const char *base, std::vector<BamChunkIndex> &idx) {
 // readers below are already filling the ring by then)
 void run_shard(Shard &sh, const MappedFile &f, Plan &plan, const ChunkPush &push, const fl_params &params, int nranks,
                const unsigned char *comm_id, const std::function<fl_ctx *()> &get_ctx0, std::atomic<bool> &abort_all, uint64_t slot_bytes,
-               bool share_kmers, bool share_contam, StreamInput *stream) {
+               bool share_kmers, const Kmers *share_contam, StreamInput *stream) {
     Ring ring;
     if (const char *e = getenv("FL_READERS")) {
         const int k = atoi(e);
@@ -284,6 +284,8 @@ void run_shard(Shard &sh, const MappedFile &f, Plan &plan, const ChunkPush &push
                 check(sh.ctx, fl_kmers_finalize(sh.ctx, &nk), "fl_kmers_finalize");
             }
             if (share_contam) {
+                if (sh.index != 0 && share_contam->contam_k() > 16)   // the table's bytes go as they are: the same size everywhere
+                    check(sh.ctx, fl_contam_configure(sh.ctx, share_contam->contam_k(), share_contam->contam_max_kmers()), "fl_contam_configure");
                 check(sh.ctx, fl_contam_broadcast(sh.ctx, 0), "fl_contam_broadcast");
                 uint64_t nk = 0;
                 check(sh.ctx, fl_contam_finalize(sh.ctx, &nk), "fl_contam_finalize");
@@ -496,13 +498,14 @@ bool score(std::vector<Shard> &shards, const Source &src, const Cuts &cuts, Plan
     const fl_params params = params_from_arguments(args);
     std::atomic<bool> abort_all(false);
     const std::function<fl_ctx *()> get_ctx0 = [&]() { return kmers.context(); };
+    const Kmers *contam = share_contam ? &kmers : nullptr;
     std::thread planner;
     if (src.growing) planner = std::thread(plan_stream, std::ref(*src.stream), src.format, std::cref(cuts), std::ref(plan));
     std::vector<std::thread> ts;
     for (int r = 1; r < nranks; ++r)
         ts.emplace_back(run_shard, std::ref(shards[r]), std::cref(*src.file), std::ref(plan), std::cref(push), std::cref(params), nranks, comm_id,
-                        std::cref(get_ctx0), std::ref(abort_all), cuts.max_chunk, share_kmers, share_contam, src.stream);
-    run_shard(shards[0], *src.file, plan, push, params, nranks, comm_id, get_ctx0, abort_all, cuts.max_chunk, share_kmers, share_contam,
+                        std::cref(get_ctx0), std::ref(abort_all), cuts.max_chunk, share_kmers, contam, src.stream);
+    run_shard(shards[0], *src.file, plan, push, params, nranks, comm_id, get_ctx0, abort_all, cuts.max_chunk, share_kmers, contam,
               src.stream);
     for (auto &t : ts) t.join();
     if (planner.joinable()) planner.join();
@@ -547,7 +550,7 @@ void finalize(std::vector<Shard> &shards, const Arguments &args, const Mark &mar
         removed_bases += (long long)s.contam.bases;
     }
     log_after_trim_split(args, n_rows, shards[0].summary);
-    if (args.contam_set) print_contam_removal(args.max_contam, removed_reads, removed_bases);
+    if (args.contam_set) print_contam_removal(args.max_contam, removed_reads, removed_bases, args.contam_k);
     log_filtering(args, shards[0].summary);
 }
 

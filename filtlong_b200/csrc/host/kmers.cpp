@@ -6,6 +6,7 @@
 #include <stdlib.h>
 
 #include <iostream>
+#include <memory>
 #include <stdexcept>
 
 #include "arena.h"
@@ -110,15 +111,17 @@ uint64_t Kmers::contam_size() {
 }
 
 // The same block as add_assembly_fasta's (kmers.cpp:61-72), then the chance that a base of random sequence lies in one
-// of the set's 16-mers: the 16-mers of a genome the size of a human one cover almost every base, which removes everything.
-void Kmers::add_contaminant_fasta(const std::string &filename) {
-    std::cerr << "Hashing 16-mers from contaminant sequences\n";
+// of the set's k-mers: 1 - (1 - n / 4^k)^k. The 16-mers of a genome the size of a human one cover almost every base, which
+// removes everything; its 31-mers cover about one base in 2^26.
+void Kmers::add_contaminant_fasta(const std::string &filename, int k) {
+    contam_k_ = k;
+    std::cerr << "Hashing " << k << "-mers from contaminant sequences\n";
     std::cerr << "  " << filename << "\n";
     const int sequence_count = add_reference(filename, false, true);
     const uint64_t n = contam_size();
     std::cerr << "  " << int_to_string(sequence_count) << " " << (sequence_count == 1 ? "contig" : "contigs") << ", "
-              << int_to_string((long long)n) << " 16-mers\n";
-    const double covered = -expm1(16.0 * log1p(-(double)n / 4294967296.0));      // 1 - (1 - n / 4^16)^16
+              << int_to_string((long long)n) << " " << k << "-mers\n";
+    const double covered = -expm1((double)k * log1p(-(double)n / ldexp(1.0, 2 * k)));
     char buf[96];
     snprintf(buf, sizeof buf, "  a random base lies in one of them with probability %.3g\n\n", covered);
     std::cerr << buf;
@@ -140,27 +143,52 @@ int Kmers::add_reference(const std::string &filename, bool multi, bool contam) {
             print_hash_progress(filename, base_count);
         }
     };
-    // the host parser over `in`, feeding packed batches (fl_kmers_add_batch)
-    auto host_parse = [&](FastxReader &in) {
+    // A contaminant set of k > 16 is a hash table sized before its first add (fl_contam_configure): by the file's bytes
+    // (after inflation), which bound its bases, when the file is in memory; otherwise by its bases, read once by the host
+    // parser into packed batches that are held until the whole input is in (a pipe cannot be read twice).
+    const bool sized = contam && contam_k_ > 16;
+    auto configure = [&](uint64_t bound) {
+        contam_max_kmers_ = bound > 0 ? bound : 1;
+        check(context(), fl_contam_configure(context(), contam_k_, contam_max_kmers_), "fl_contam_configure");
+    };
+    // the host parser over `in`, feeding packed batches (fl_kmers_add_batch); hold_all: size the set first (see above)
+    auto host_parse = [&](FastxReader &in, bool hold_all) {
         const uint64_t kBatchBases = 256ull << 20;
-        HostArena arena(true, false, true);
-        auto flush = [&]() {
-            if (arena.empty()) return;
-            fl_batch b = arena.batch();
+        std::vector<std::unique_ptr<HostArena>> held;
+        auto arena = std::make_unique<HostArena>(true, false, true);
+        auto add = [&](const HostArena &a) {
+            fl_batch b = a.batch();
             fl_ctx *c = context();
             if (contam) check(c, fl_contam_add_batch(c, &b), "fl_contam_add_batch");
             else check(c, fl_kmers_add_batch(c, &b, multi ? 1 : 0), "fl_kmers_add_batch");
-            arena.clear();
+        };
+        auto flush = [&]() {
+            if (arena->empty()) return;
+            if (hold_all) {
+                held.push_back(std::move(arena));
+                arena = std::make_unique<HostArena>(true, false, true);
+                return;
+            }
+            add(*arena);
+            arena->clear();
         };
         while (in.ok() && in.next() >= 0) {        // a parse error silently ends hashing (kmers.cpp:90-94)
             ++sequence_count;
             if (in.seq.size() < 16) continue;      // kmers.cpp:99-100
             base_count += (long long)in.seq.size();
-            arena.add(in.seq.data(), nullptr, (int64_t)in.seq.size());
-            if (arena.padded_bases() >= kBatchBases) flush();
+            arena->add(in.seq.data(), nullptr, (int64_t)in.seq.size());
+            if (arena->padded_bases() >= kBatchBases) flush();
             progress(false);
         }
         flush();
+        if (!hold_all) return;
+        uint64_t bases = 0;
+        for (const auto &a : held) bases += a->bases();
+        configure(bases);
+        for (auto &a : held) {
+            add(*a);
+            a.reset();
+        }
     };
     MappedFile f;
     std::vector<Chunk> plan;
@@ -176,6 +204,7 @@ int Kmers::add_reference(const std::string &filename, bool multi, bool contam) {
     }
     if (text_path) {
         fl_ctx *c = context();
+        if (sized) configure(f.size);
         for (size_t i = 0; i < plan.size(); ++i) {
             const Chunk &ch = plan[i];
             uint64_t n_rec = 0, n_bases = 0, used = 0;
@@ -197,7 +226,7 @@ int Kmers::add_reference(const std::string &filename, bool multi, bool contam) {
             if (used != ch.end - ch.begin) {                            // the host reader takes over at the first byte not consumed
                 if (timing) std::cerr << (last_progress ? "\n" : "") << "[timing] reference " << filename << ": host reader from byte " << ch.begin + used << "\n";
                 FastxReader in(f.base + ch.begin + used, f.size - ch.begin - used);
-                host_parse(in);
+                host_parse(in, false);
                 break;
             }
             if (timing && i + 1 == plan.size())
@@ -206,7 +235,7 @@ int Kmers::add_reference(const std::string &filename, bool multi, bool contam) {
     } else {
         if (timing) std::cerr << "[timing] reference " << filename << ": host reader\n";
         FastxReader in(filename);
-        host_parse(in);
+        host_parse(in, sized);
     }
     progress(true);
     std::cerr << "\n";

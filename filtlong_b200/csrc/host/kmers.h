@@ -33,8 +33,11 @@ public:
     uint64_t size();               // m_kmers.size()
     fl_ctx *context();
     // --contam: the contaminant set on the same context, built like add_assembly_fasta's set, with its log block
-    void add_contaminant_fasta(const std::string &filename);
+    // k: the contaminant k-mers' length (--contam_k); the set's table is sized by the file's bases (fl_contam_configure)
+    void add_contaminant_fasta(const std::string &filename, int k = 16);
     uint64_t contam_size();        // 0 when none was added
+    int contam_k() const { return contam_k_; }
+    uint64_t contam_max_kmers() const { return contam_max_kmers_; }   // what fl_contam_configure was given
 
     // fl_gzip_inflate on context(), for inflate_gzip_memory (gzmem.h): tried on gzip input that is not BGZF and has at
     // least kDeviceGunzipMinBytes compressed bytes; a decline or a CUDA failure leaves the file to the host z_stream.
@@ -47,4 +50,6 @@ private:
     int add_reference(const std::string &filename, bool require_multiple_copies, bool contam = false);
     fl_ctx *ctx_ = nullptr;
     int device_ = 0;
+    int contam_k_ = 16;
+    uint64_t contam_max_kmers_ = 0;
 };

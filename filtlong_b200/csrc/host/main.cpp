@@ -83,7 +83,7 @@ int main(int argc, char **argv) {
         if (args.assembly_set) kmers.add_assembly_fasta(args.assembly);
         if (!args.short_reads.empty()) kmers.add_read_fastqs(args.short_reads);
         const bool kmers_empty = kmers.empty();
-        if (args.contam_set) kmers.add_contaminant_fasta(args.contam);   // after -1/-2, whose build state is released by now
+        if (args.contam_set) kmers.add_contaminant_fasta(args.contam, args.contam_k);   // after -1/-2, whose build state is released by now
         timer.mark("reference k-mers (+ CUDA init)");
 
         // ---- the device feeder ----
@@ -200,7 +200,7 @@ int main(int argc, char **argv) {
             for (size_t row = 0; row < reads.n_rows(); ++row)
                 if (reads.ranked(row)) longest_read_name = std::max(longest_read_name, reads.row_name(row).size());
         log_after_trim_split(args, reads.n_rows() - reads.contam.rows, summary);
-        if (args.contam_set) print_contam_removal(args.max_contam, (long long)reads.contam.reads, (long long)reads.contam.bases);
+        if (args.contam_set) print_contam_removal(args.max_contam, (long long)reads.contam.reads, (long long)reads.contam.bases, args.contam_k);
         if (args.verbose) {
             std::cerr << "\n\n" << "Read name" << "\t" << "Length score" << "\t" << "Mean quality score" << "\t"
                       << "Window quality score" << "\t" << "Final score" << "\n";

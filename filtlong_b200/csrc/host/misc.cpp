@@ -32,10 +32,10 @@ void print_read_score_progress(long long read_count, long long base_count) {
     std::cerr << "\r  " << int_to_string(read_count) << " reads (" << int_to_string(base_count) << " bp)";
 }
 
-void print_contam_removal(double max_contam, long long reads, long long bases) {
+void print_contam_removal(double max_contam, long long reads, long long bases, int k) {
     std::ostringstream pct;
     pct << max_contam;
     std::cerr << "Removing contaminant reads\n";
     std::cerr << "  " << int_to_string(reads) << " reads (" << int_to_string(bases) << " bp) with more than " << pct.str()
-              << "% of bases in contaminant 16-mers\n\n";
+              << "% of bases in contaminant " << k << "-mers\n\n";
 }

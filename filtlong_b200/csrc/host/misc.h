@@ -8,4 +8,4 @@ std::string int_to_string(long long n);          // digit grouping of the user's
 void print_hash_progress(const std::string &filename, long long base_count);
 void print_read_score_progress(long long read_count, long long base_count);
 // --contam: "Removing contaminant reads" and the removed reads and bases (nothing without --contam)
-void print_contam_removal(double max_contam, long long reads, long long bases);
+void print_contam_removal(double max_contam, long long reads, long long bases, int k);

@@ -187,8 +187,28 @@ int fl_contam_add_text(fl_ctx *ctx, const char *host_text, uint64_t n_bytes, int
 int fl_contam_add_batch(fl_ctx *ctx, const fl_batch *host_batch);
 int fl_contam_finalize(fl_ctx *ctx, uint64_t *n_kmers_out);
 int fl_contam_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out);
-/* collective, like fl_kmers_broadcast */
+/* collective, like fl_kmers_broadcast. A set of k > 16 goes as its table's bytes: every rank must have called
+ * fl_contam_configure with the same k and max_kmers. The ranks first compare k and the table size; when any differs,
+ * every rank returns FL_EINVAL and nothing is sent. */
 int fl_contam_broadcast(fl_ctx *ctx, int root);
+/* Not a reference option (--contam_k): the contaminant set's k-mer length, 16 to 32 (16 = the set above, the default).
+ * Call before the first contaminant add and before any read is pushed (FL_EINVAL after either, or for k outside 16..32).
+ * For k > 16 the set is a device hash set of canonical k-mers, sized here for at most max_kmers of them (a bound on the
+ * contaminant's bases will do): 32 bytes per 3.2 k-mers, rounded up to a power of two; FL_ENOMEM, with the GiB it needed
+ * in the message, when the device lacks the memory. Every window of k bases of a contaminant record that holds only ACGTacgt
+ * adds min(forward, reverse complement); a window with any other character adds nothing. An add that could take the set
+ * past its reservation is FL_EINVAL and adds nothing. A read's k-mers come from its 2-bit codes (a non-ACGT base is A), and a
+ * base is covered when a k-mer containing it is in the set on either strand. fl_contam_finalize then counts the forward and
+ * reverse k-mers: 2 * canonical - palindromes. */
+int fl_contam_configure(fl_ctx *ctx, int k, uint64_t max_kmers);
+/* k > 16: the canonical members in any order (at most cap; *n_out = how many there are). fl_contam_export is FL_EINVAL then. */
+int fl_contam_export64(fl_ctx *ctx, uint64_t *out, uint64_t cap, uint64_t *n_out);
+/* k > 16: out[i] = the forward k-mer fwd_kmers[i] (2-bit codes, first base in the high bits) is in the set on either strand */
+int fl_contam_contains64(fl_ctx *ctx, const uint64_t *fwd_kmers, uint32_t n, uint8_t *out);
+/* k > 16, for measurement: hist[0, n_bins) counts members by the buckets (32-byte sectors) a look-up of them reads,
+ * hist[n_bins, 2 * n_bins) counts buckets by the sectors a look-up of an absent k-mer hashed there reads; the last bin of
+ * each holds that many or more. */
+int fl_contam_probe_lengths(fl_ctx *ctx, uint64_t *hist, int n_bins);
 typedef struct fl_contam_counts {
     uint64_t reads;    /* input reads removed */
     int64_t bases;     /* their bases */
