@@ -1,11 +1,35 @@
-"""Helpers of the BGZF tests: synthetic FASTQ / FASTA corpora, zlib's BGZF of the same blocks, member walking."""
+"""Helpers of the BGZF tests: synthetic FASTQ / FASTA corpora, zlib's BGZF of the same blocks, member walking, and the
+host build of the kernel's Huffman / CRC arithmetic (tests/bgzf_codes_dump.cpp over fl_bgzf.h)."""
+import os
 import struct
+import subprocess
 import zlib
 
 import numpy as np
 
 BLOCK = 0xff00
 EOF_MEMBER = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CSRC = os.path.join(ROOT, "filtlong_b200", "csrc")
+
+
+def build_codes_dumper(out_dir):
+    """Compiles tests/bgzf_codes_dump.cpp (fl_bgzf.h for the host) into out_dir; returns the executable's path."""
+    out = os.path.join(str(out_dir), "bgzf_codes_dump")
+    r = subprocess.run(["g++", "-std=c++17", "-O2", "-I", CSRC, os.path.join(ROOT, "tests", "bgzf_codes_dump.cpp"), "-o", out],
+                       capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    return out
+
+
+def huff_codes(dumper, freqs, maxbits):
+    """fl_huff_lengths_sorted over the used symbols in ascending (frequency, symbol) order, then fl_huff_canonical:
+    (lengths, bit-reversed codes), one entry per symbol of freqs."""
+    r = subprocess.run([dumper, "huff", str(maxbits), str(len(freqs))] + [str(int(f)) for f in freqs],
+                       capture_output=True, text=True, check=True)
+    lines = r.stdout.split("\n")
+    return [int(x) for x in lines[0].split()], [int(x) for x in lines[1].split()]
 
 
 def ont_header(rng, i):

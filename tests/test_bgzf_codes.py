@@ -2,31 +2,22 @@
 code lengths and canonical codes on random and adversarial histograms, and the CRC-32 of a block assembled from its
 threads' slices."""
 import heapq
-import os
 import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "filtlong_b200", "csrc")
+from tests import bgzf_util as bu
 
 
 @pytest.fixture(scope="module")
 def dumper(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("bgzf") / "bgzf_codes_dump")
-    r = subprocess.run(["g++", "-std=c++17", "-O2", "-I", CSRC, os.path.join(ROOT, "tests", "bgzf_codes_dump.cpp"), "-o", out],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return out
+    return bu.build_codes_dumper(tmp_path_factory.mktemp("bgzf"))
 
 
 def codes(dumper, freqs, maxbits):
-    r = subprocess.run([dumper, "huff", str(maxbits), str(len(freqs))] + [str(int(f)) for f in freqs],
-                       capture_output=True, text=True, check=True)
-    lines = r.stdout.split("\n")
-    return [int(x) for x in lines[0].split()], [int(x) for x in lines[1].split()]
+    return bu.huff_codes(dumper, freqs, maxbits)
 
 
 def huffman_cost(freqs):
