@@ -195,12 +195,17 @@ __device__ __forceinline__ void score_fused(const PhredArgs &a, uint32_t r, cons
     finish(a, r, L, sum, best);
 }
 
-__device__ __forceinline__ int n_segments(int L, int ws) { return (L - ws + PH_SEG - 1) / PH_SEG; }
+// Window sizes reach 2^31 - 1, so sums like ws + PH_SEG can wrap in int: these are written as differences, which cannot
+// (L >= 0, ws > 0). A segmented read has L - ws > PH_SEG.
+__device__ __forceinline__ int n_segments(int L, int ws) { return (L - ws - 1) / PH_SEG + 1; }
 
 __device__ __forceinline__ unsigned long long items_of(int L, int ws) {
-    if (L <= PH_LONG || L <= ws + PH_SEG) return 1ull;
+    if (L <= PH_LONG || L - ws <= PH_SEG) return 1ull;
     return 1ull + (unsigned long long)n_segments(L, ws);
 }
+
+// end of the segment that starts at P < L
+__device__ __forceinline__ int segment_end(int P, int L) { return (L - P > PH_SEG) ? P + PH_SEG : L; }
 
 // one segment of the window chain of a long read, from a predicted entry value
 __device__ __forceinline__ void score_segment(const PhredArgs &a, uint32_t r, int seg, size_t idx, const Tab &t) {
@@ -209,8 +214,8 @@ __device__ __forceinline__ void score_segment(const PhredArgs &a, uint32_t r, in
     double sum = 0.0, w = 0.0, best = 0.0;
     chain<true, false>(q, 0, ws, ws, t, sum, w, best);
     const double w0 = sum / (double)ws;              // exact first window (read.cpp:220-223)
-    const int P = ws + seg * PH_SEG;
-    const int Pend = (P + PH_SEG < L) ? P + PH_SEG : L;
+    const int P = ws + seg * PH_SEG;                 // < L: no wrap
+    const int Pend = segment_end(P, L);
     double entry = w0;
     if (seg > 0) {
         // prediction: grid steps of w inside the binade of w0 (see the file header)
@@ -432,7 +437,8 @@ __global__ void k_phred_fill(const int32_t *__restrict__ len, uint32_t n, int ws
     for (int k = 0; k < cnt - 1; ++k) {
         items[base + 1 + k] = make_uint2(r, (uint32_t)k);
         const int P = ws + k * PH_SEG;
-        cost[base + 1 + k] = 1 * 256 + fl_length_bucket(((P + PH_SEG < L) ? PH_SEG : L - P) + 2 * ws);
+        const long long work = (long long)(segment_end(P, L) - P) + 2ll * ws;   // 2 * ws alone can pass INT_MAX
+        cost[base + 1 + k] = 1 * 256 + fl_length_bucket(work < INT_MAX ? (int)work : INT_MAX);
     }
 }
 

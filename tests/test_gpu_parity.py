@@ -90,10 +90,12 @@ def test_phred_long_reads_and_batches():
 
 @pytest.mark.parametrize("ws", [250, 16, 1000])
 def test_phred_long_read_segment_prediction_and_fallback(ws):
-    """Long reads are cut into segments whose entry value of the window recurrence is PREDICTED and
-    then verified (fl_phred.cu). These reads make the prediction fail on purpose -- the window
-    quality crosses binades (0.99 -> 0.2 -> 0.99), window sizes with round-to-even ties (16), bytes
-    outside the Phred range -- so the serial re-score path must produce the reference's bits too."""
+    """Under the work-item kernels (fl_phred.cu), long reads are cut into segments whose entry value of
+    the window recurrence is PREDICTED and then verified. These reads make the prediction fail on
+    purpose -- the window quality crosses binades (0.99 -> 0.2 -> 0.99), bytes outside the Phred
+    range -- so the serial re-score path must produce the reference's bits too. Only ws = 1000 takes
+    that path: 250 and 16 are scored by the lattice kernels (k_phred_sum / k_phred_win) and check
+    those on the same reads. tests/test_gpu_phred_items.py aims at the work-item path's seams."""
     rng = np.random.default_rng(99)
     reads = []
     reads.append((b"A" * 120000, b"I" * 50000 + b"#" * 30000 + b"I" * 40000))                  # binade crossings

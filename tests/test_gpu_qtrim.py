@@ -54,12 +54,18 @@ CASES = [
     (10, False, 32, 300, 2, dict(keep_percent=60.0, min_window_q=5.0)),
     (7, True, 500, 300, 1, dict(keep_percent=50.0)),
     (20, True, 1, 100, 1, dict(min_length=100)),
+    # window sizes the work-item kernels score; max_len (not a threshold) makes parents long enough that children of more
+    # than PH_LONG = 24576 bases are cut into window segments
+    (20, True, 16, 7, 1, dict(keep_percent=80.0)),
+    (10, True, 500, 1000, 2, dict(keep_percent=70.0, max_len=100000)),
 ]
 
 
 @pytest.mark.parametrize("Q,trim,split,ws,pushes,thr", CASES, ids=lambda x: str(x))
 def test_rows_and_scores_equal_the_model(Q, trim, split, ws, pushes, thr):
-    reads = reads_with_bad_blocks(100 + Q + ws, 150)
+    thr = dict(thr)
+    max_len = thr.pop("max_len", None)
+    reads = reads_with_bad_blocks(100 + Q + ws, 150, **({"max_len": max_len} if max_len else {}))
     kw = dict(window_size=ws, trim=trim, split=split, **thr)
     ctx, summary = run_ctx(reads, dict(kw, trim_q=Q), pushes)
     sc = qm.score_rows(reads, Q, kw)
@@ -70,6 +76,8 @@ def test_rows_and_scores_equal_the_model(Q, trim, split, ws, pushes, thr):
     parity.check_rescale_exact(rw, summary, p)
     parity.check_selection_exact(rw, summary, p)
     assert sum(len(k) for k in sc.children) > len(reads) // 4          # the case does split reads
+    if max_len:
+        assert max(c.end - c.start for k in sc.children for c in k) > 24576
     ctx.close()
 
 
