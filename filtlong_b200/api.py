@@ -96,7 +96,7 @@ class Context:
         return int(self.L.fl_ctx_launch_count(self.h))
 
     KERNELS = {"score_phred": 0, "probe_paint": 1, "kmer_stats": 2, "kmers_add": 3,
-               "qual_mask": 4, "row_scan": 5, "qual_gather": 6, "qual_children": 7, "contam": 8}
+               "qual_mask": 4, "row_scan": 5, "qual_gather": 6, "qual_children": 7, "contam": 8, "bam_build": 9, "bgzf": 10}
 
     def enable_timing(self, on=True):
         self._ck(self.L.fl_ctx_enable_timing(self.h, int(on)), "fl_ctx_enable_timing")
@@ -341,6 +341,26 @@ class Context:
         self._ck(rc, "fl_bgzf_compress_device")
         return m.value
 
+    # ---- BAM output (fl_bam_build) ----
+    def bam_build(self, batch, items, keep_mods=False):
+        """The uncompressed BAM records of items over the bytes `batch`: items are (off, s, e) -- s < 0 copies bytes
+        [off, off + e), else the child [s, e) of the record at off. Returns (bytes, [kept, invalid])."""
+        src = np.frombuffer(batch, dtype=np.uint8)
+        it = bam_items(items)
+        counts = np.zeros(2, np.uint64)
+        n = C.c_uint64()
+        cap = 0
+        while True:
+            out = np.empty(max(cap, 1), dtype=np.uint8)
+            rc = self.L.fl_bam_build(self.h, capi.ptr(src), src.size, capi.ptr(it), it.size, int(keep_mods), capi.ptr(out), cap,
+                                     C.byref(n), capi.ptr(counts))
+            if rc != capi.FL_ERANGE:
+                break
+            cap = n.value
+            counts[:] = 0
+        self._ck(rc, "fl_bam_build")
+        return out[:n.value].tobytes(), [int(x) for x in counts]
+
     def row_results(self):
         _, n, _ = self.counts()
         m = max(n, 1)
@@ -351,6 +371,45 @@ class Context:
         o = capi.RowResults(**{k: capi.ptr(v) for k, v in r.items()})
         self._ck(self.L.fl_results_rows(self.h, C.byref(o)), "fl_results_rows")
         return {k: v[:n] for k, v in r.items()}
+
+
+def bam_items(items):
+    """(off, s, e) tuples as an array of fl_bam_item"""
+    it = np.zeros(len(items), dtype=[("off", "<u8"), ("s", "<i4"), ("e", "<i4")])
+    for k, (o, s_, e_) in enumerate(items):
+        it[k] = (o, s_, e_)
+    return it
+
+
+class BamWriter:
+    """fl_bam_writer on a context: one BGZF-compressed BAM stream, built and compressed batch by batch."""
+
+    def __init__(self, ctx):
+        self.ctx, self.h = ctx, C.c_void_p()
+        ctx._ck(ctx.L.fl_bam_writer_create(ctx.h, C.byref(self.h)), "fl_bam_writer_create")
+
+    def push(self, batch, items, keep_mods=False, last=False):
+        """fl_bam_writer_push: the members of the whole blocks so far (all of them when last), and [kept, invalid]"""
+        src = np.frombuffer(batch, dtype=np.uint8)
+        it = bam_items(items)
+        cap = int(self.ctx.L.fl_bgzf_bound(capi.FL_BGZF_BLOCK + 2 * src.size + 300 * len(items)))
+        n = C.c_uint64()
+        while True:                          # a push that does not fit changes nothing but the counts: again, with room
+            out = np.empty(max(cap, 1), dtype=np.uint8)
+            counts = np.zeros(2, np.uint64)
+            rc = self.ctx.L.fl_bam_writer_push(self.h, capi.ptr(src), src.size, capi.ptr(it), it.size, int(keep_mods), int(last),
+                                               capi.ptr(out), cap, C.byref(n), capi.ptr(counts))
+            if rc != capi.FL_ERANGE:
+                break
+            cap = n.value
+        self.ctx._ck(rc, "fl_bam_writer_push")
+        return out[:n.value].tobytes(), [int(x) for x in counts]
+
+    def close(self):
+        if self.h:
+            self.ctx.L.fl_bam_writer_destroy(self.h)
+            self.h = None
+
 
 
 def bgzf_compress(data, append_eof=True, device=0):

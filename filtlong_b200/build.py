@@ -13,7 +13,7 @@ BUILD = os.path.join(PKG, "build")
 LIB = os.path.join(PKG, "libfiltlong_b200.so")
 SOURCES = ["fl_api.cu", "fl_scan.cu", "fl_kmers.cu", "fl_score.cu", "fl_phred.cu", "fl_qtrim.cu", "fl_select.cu", "fl_comm.cu", "fl_text.cu", "fl_synth.cu",
            "fl_contam_k.cu", "fl_bgzf.cu", "fl_bam.cu", "fl_inflate.cu", "fl_synth_host.cpp"]
-HEADERS = ["fl_internal.cuh", "fl_device.cuh", "fl_synth.h", "fl_bgzf.h", "fl_inflate.h", "fl_name_hash.h", os.path.join("..", "..", "include", "filtlong_b200.h")]
+HEADERS = ["fl_internal.cuh", "fl_device.cuh", "fl_synth.h", "fl_bgzf.h", "fl_bam_mods.h", "fl_inflate.h", "fl_name_hash.h", os.path.join("..", "..", "include", "filtlong_b200.h")]
 # host-only synthetic generators on their own (no CUDA inside): what bench.py's CPU legs load
 SYNTH_LIB = os.path.join(PKG, "libflsynth_host.so")
 CXX = os.environ.get("CXX", "g++")

@@ -207,6 +207,11 @@ SYMBOLS = [
     ("fl_synth_assembly_host", None, [C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint32, _P, _P]),
     ("fl_synth_ascii_device", C.c_int, [_P, C.c_uint32, _P, _P, _P, _P, _P]),
     ("fl_synth_ascii_host", None, [C.c_uint32, _P, _P, _P, _P, _P]),
+    ("fl_bam_build", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, _P, C.c_uint64, C.POINTER(C.c_uint64), _P]),
+    ("fl_bam_build_device", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, _P, C.c_uint64, C.POINTER(C.c_uint64), _P]),
+    ("fl_bam_writer_create", C.c_int, [_P, C.POINTER(_P)]),
+    ("fl_bam_writer_push", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.c_int, _P, C.c_uint64, C.POINTER(C.c_uint64), _P]),
+    ("fl_bam_writer_destroy", None, [_P]),
     ("fl_bgzf_bound", C.c_uint64, [C.c_uint64]),
     ("fl_bgzf_compress", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
     ("fl_bgzf_compress_device", C.c_int, [_P, _P, C.c_uint64, _P, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),

@@ -449,6 +449,7 @@ int bgzf_run(fl_ctx *c, const uint8_t *din, uint64_t n, uint8_t *dout, uint64_t 
         }
     }
     for (uint64_t b0 = 0; b0 < blocks; b0 += chunk) {
+        KernelTimer kt(c, FL_KERNEL_BGZF);
         const uint32_t m = (uint32_t)(blocks - b0 < chunk ? blocks - b0 : chunk);
         k_bgzf_deflate<<<m, BZ_THREADS, SM_BYTES, s>>>(din, n, b0, c->bz_slots.p, c->bz_sizes.p);
         k_bgzf_offsets<<<1, 1024, 0, s>>>(c->bz_sizes.p, m, c->bz_offs.p, c->bz_state.p);

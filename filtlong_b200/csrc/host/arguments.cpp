@@ -124,6 +124,7 @@ const Opt kOpts[] = {
     {0, "trim", false, "trim", "trim non-k-mer-matching bases from start/end of reads"},
     {0, "split", true, "split", "split reads at this many (or more) consecutive non-k-mer-matching bases (unit suffixes: k, kb, m, mb, g, gb)"},
     {0, "trim_q", true, "int", "without a reference, --trim / --split on Phred scores: a base is good if it lies in 16 consecutive bases of at least this quality (1 to 93; not a reference option)"},
+    {0, "keep_mods", false, "keep_mods", "BAM input: trimmed and split reads keep the base-modification tags (MM/ML) that fall inside them, re-based (not a reference option)"},
     {0, "window_size", true, "int", "size of sliding window used when measuring window quality (default: 250)"},
     {0, "gpus", true, "int", "number of GPUs to shard the read set across (default: 1; not a reference option)"},
     {0, "bgzip", false, "bgzip", "compress the output as BGZF (gzip-compatible) on the GPU (not a reference option)"},
@@ -144,8 +145,8 @@ void print_help(const char *prog) {
         {"external references (if provided, read quality will be determined using these instead of from the Phred scores):", 6, 8},
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
         {"contaminant removal:", 12, 14},
-        {"read manipulation:", 15, 17},
-        {"other:", 18, 24},
+        {"read manipulation:", 15, 18},
+        {"other:", 19, 25},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -191,6 +192,7 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "trim") trim = true;
         else if (ln == "split") { split = read_int_suffix(nm, v); split_set = true; }
         else if (ln == "trim_q") trim_q = read_trim_q(v);
+        else if (ln == "keep_mods") keep_mods = true;
         else if (ln == "window_size") window_ll = read_plain_ll(nm, v);
         else if (ln == "gpus") gpus = (int)read_plain_ll(nm, v);
         else if (ln == "bgzip") bgzip = true;
@@ -264,6 +266,7 @@ Arguments::Arguments(int argc, char **argv) {
     const bool some_reference = !short_reads.empty() || assembly_set;
     if (trim_q > 0 && some_reference) FAIL("Error: --trim_q cannot be used with an assembly or read reference");
     if (trim_q > 0 && !trim && !split_set) FAIL("Error: --trim_q needs --trim or --split");
+    if (keep_mods && !trim && !split_set) FAIL("Error: --keep_mods needs --trim or --split");
     if (trim && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --trim");
     if (split_set && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --split");
     if (max_contam_set && !contam_set) FAIL("Error: --max_contam needs --contam");

@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <stdexcept>
 
+#include "../fl_bam_mods.h"
 #include "../fl_name_hash.h"
 
 namespace {
@@ -26,40 +27,11 @@ inline uint16_t u16(const char *p) {
     return v;
 }
 
-// size of one value of an aux type ('B' arrays: of one element), 0 for a type that is not one
-int aux_size(char t) {
-    switch (t) {
-    case 'A': case 'c': case 'C': return 1;
-    case 's': case 'S': return 2;
-    case 'i': case 'I': case 'f': return 4;
-    default: return 0;
-    }
-}
-
 // the aux field at p (tag, type, value) ends at *next, not after `end`; false if it does not parse
 bool aux_field(const char *p, const char *end, const char **next) {
-    if (end - p < 3) return false;
-    const char t = p[2];
-    p += 3;
-    if (t == 'Z' || t == 'H') {
-        const void *z = memchr(p, 0, (size_t)(end - p));
-        if (!z) return false;
-        *next = (const char *)z + 1;
-        return true;
-    }
-    if (t == 'B') {
-        if (end - p < 5) return false;
-        const int s = aux_size(p[0]);
-        if (!s || p[0] == 'A') return false;
-        const uint64_t n = u32(p + 1);
-        if ((uint64_t)(end - p - 5) < n * (uint64_t)s) return false;
-        *next = p + 5 + n * (uint64_t)s;
-        return true;
-    }
-    const int s = aux_size(t);
-    if (!s || end - p < s) return false;
-    *next = p + s;
-    return true;
+    const uint8_t *n = fl_aux_next((const uint8_t *)p, (const uint8_t *)end);
+    if (n) *next = (const char *)n;
+    return n != nullptr;
 }
 
 std::string at_byte(uint64_t off) { return "record at byte " + std::to_string(off); }
@@ -93,9 +65,9 @@ bool bam_header(const char *b, uint64_t size, uint64_t *end, std::string *why) {
 }
 
 bool bam_plan_chunks(const char *b, uint64_t size, uint64_t header_end, uint64_t target, std::vector<Chunk> &out, uint64_t *max_chunk,
-                     std::string *why) {
+                     std::string *why, uint64_t *max_record) {
     const uint64_t kMaxChunk = (1ull << 31) - 1;
-    uint64_t p = header_end, lo = header_end, biggest = 0;
+    uint64_t p = header_end, lo = header_end, biggest = 0, biggest_record = 0;
     auto cut = [&](uint64_t e) {
         out.push_back(Chunk{lo, e});
         biggest = std::max(biggest, e - lo);
@@ -108,11 +80,13 @@ bool bam_plan_chunks(const char *b, uint64_t size, uint64_t header_end, uint64_t
         if (bs + 4 > size - p) { *why = "malformed BAM input: " + at_byte(p) + " runs past the end of the file"; return false; }
         if (bs + 4 > kMaxChunk) { *why = "BAM " + at_byte(p) + " is larger than 2 GiB"; return false; }
         const uint64_t e = p + 4 + bs;
+        biggest_record = std::max(biggest_record, 4 + bs);
         if (e - lo > target && p > lo) cut(p);                              // the record starts the next chunk
         p = e;
     }
     if (p > lo) cut(p);
     *max_chunk = biggest;
+    if (max_record) *max_record = biggest_record;
     return true;
 }
 
@@ -173,8 +147,9 @@ bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix) {
 }
 
 uint64_t bam_record_bytes(const char *rec) { return 4 + (uint64_t)u32(rec); }
+uint32_t bam_l_seq(const char *rec) { return u32(rec + kLSeq); }
 
-void bam_child_record(const char *rec, int start, int end, std::string &out) {
+int bam_child_record(const char *rec, int start, int end, std::string &out, bool keep_mods) {
     const uint64_t l_name = (uint8_t)rec[kLReadName], n_cigar = u16(rec + kNCigar), l_seq = u32(rec + kLSeq);
     const char *name = rec + kFixed, *seq = name + l_name + 4 * n_cigar, *qual = seq + (l_seq + 1) / 2, *rec_end = rec + bam_record_bytes(rec);
     std::string nm(name, l_name - 1);
@@ -197,12 +172,59 @@ void bam_child_record(const char *rec, int start, int end, std::string &out) {
     }
     if (bam_no_quality(qual)) out.append(n, (char)0xFF);
     else out.append(qual + start, n);
-    for (const char *a = qual + l_seq; a < rec_end;) {                        // of the aux fields only RG
+    for (const char *a = qual + l_seq; a < rec_end;) {                        // the RG fields, then the modification tags
         const char *next = rec_end;
         aux_field(a, rec_end, &next);
         if (a[0] == 'R' && a[1] == 'G') out.append(a, (size_t)(next - a));
         a = next;
     }
+    int status = 0;
+    FlModTags t;
+    fl_mod_tags((const uint8_t *)qual + l_seq, (const uint8_t *)rec_end, (int64_t)l_seq, &t);
+    if (keep_mods && t.has_mm) {
+        uint64_t total[5] = {0, 0, 0, 0, l_seq}, before_s[5] = {0, 0, 0, 0, (uint64_t)start}, before_e[5] = {0, 0, 0, 0, (uint64_t)end};
+        for (uint32_t i = 0; i < l_seq; ++i)
+            for (int b = 0; b < 4; ++b)
+                if (nib(i) == fl_mm_code(b)) {
+                    ++total[b];
+                    before_s[b] += i < (uint32_t)start;
+                    before_e[b] += i < (uint32_t)end;
+                }
+        status = FL_BAM_MODS_INVALID;
+        if (fl_mods_valid(t, total)) {
+            status = FL_BAM_MODS_KEPT;
+            std::string mm, ml;
+            uint64_t ml_at = 0, calls;
+            for (uint32_t p = 0; p < t.mm_len;) {
+                uint32_t head, codes;
+                int b;
+                fl_mm_head(t.mm, t.mm_len, p, &head, &b, &codes);
+                mm.append((const char *)t.mm + p, head);
+                FlMMCursor cur = fl_mm_cursor(p + head);
+                std::string deltas(t.mm_len, '\0');                                 // no longer than the parent's
+                uint64_t k0, k1;
+                deltas.resize(fl_mm_rebase(t.mm, t.mm_len, cur, before_s[b], before_e[b], (uint8_t *)&deltas[0], &k0, &k1));
+                mm += deltas;
+                mm += ';';
+                if (t.has_ml) ml.append((const char *)t.ml + ml_at + k0 * codes, (size_t)((k1 - k0) * codes));
+                p = fl_mm_group_end(t.mm, cur, &calls);
+                ml_at += calls * codes;
+            }
+            std::string mm_field = "MMZ" + mm;
+            mm_field += '\0';
+            std::string ml_field;
+            if (t.has_ml) {
+                const uint32_t k = (uint32_t)ml.size();
+                ml_field = "MLBC";
+                ml_field.append((const char *)&k, 4);
+                ml_field += ml;
+            }
+            out += t.ml_first ? ml_field + mm_field : mm_field + ml_field;
+            out += "MNI";
+            out.append((const char *)&n, 4);
+        }
+    }
     const uint32_t bs = (uint32_t)(out.size() - at - 4);
     memcpy(&out[at], &bs, 4);
+    return status;
 }

@@ -30,9 +30,9 @@ bool bam_header(const char *b, uint64_t size, uint64_t *end, std::string *why);
 
 // The records after the header in chunks of whole records of at most `target` bytes; a record larger than that is a
 // chunk of its own, and no chunk reaches 2 GiB. Checks the block_size chain: every block_size >= 32, every record ends
-// inside the input. *max_chunk: the largest chunk.
+// inside the input. *max_chunk: the largest chunk; *max_record (when given): the largest record.
 bool bam_plan_chunks(const char *b, uint64_t size, uint64_t header_end, uint64_t target, std::vector<Chunk> &out, uint64_t *max_chunk,
-                     std::string *why);
+                     std::string *why, uint64_t *max_record = nullptr);
 
 // One chunk's records, offsets relative to the chunk's first byte. seq32 / qual32: the same offsets as rec.seq_off /
 // rec.qual_off, in the width fl_reads_push_bam takes.
@@ -50,10 +50,14 @@ bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix);
 // the record whose read_name starts at `name`: its first byte (block_size) and its size
 inline const char *bam_record_of(const char *name) { return name - 36; }
 uint64_t bam_record_bytes(const char *rec);
+uint32_t bam_l_seq(const char *rec);
 // QUAL of the record starts with 0xFF: the record has no quality
 inline bool bam_no_quality(const char *qual) { return (unsigned char)qual[0] == 0xFF; }
 
 // Appends to `out` the record of a child [start, end) of `rec` (0 <= start < end <= l_seq): the parent's fixed fields,
 // read_name name_<start+1>-<end>, SEQ and QUAL of the slice (QUAL all 0xFF when the parent has none), and of the aux
-// fields only the parent's RG. Throws std::runtime_error when the child's name does not fit in a BAM record.
-void bam_child_record(const char *rec, int start, int end, std::string &out);
+// fields the parent's RG; with keep_mods, when the parent's MM / ML / MN are valid, then its MM and ML re-based to the
+// child (fl_bam_mods.h) and MN:I = end - start. Throws std::runtime_error when the child's name does not fit in a BAM
+// record. Returns FL_BAM_MODS_KEPT, FL_BAM_MODS_INVALID (keep_mods, the parent has an MM tag and its tags are not
+// valid) or 0.
+int bam_child_record(const char *rec, int start, int end, std::string &out, bool keep_mods = false);

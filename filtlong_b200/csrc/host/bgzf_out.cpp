@@ -7,6 +7,8 @@
 #include <algorithm>
 #include <stdexcept>
 
+#include "bam.h"
+
 namespace {
 
 // the empty member that ends a BGZF file (SAM specification 4.1.2)
@@ -28,9 +30,18 @@ bool write_all(int fd, const char *p, uint64_t n) {
 
 }  // namespace
 
-BgzfOut::BgzfOut(fl_ctx *ctx, int fd) : ctx_(ctx), fd_(fd) {
+BgzfOut::BgzfOut(fl_ctx *ctx, int fd, const BamOut *bam) : ctx_(ctx), fd_(fd) {
     in_cap_ = 1028ull * FL_BGZF_BLOCK;                     // 64 MiB of input per batch
     out_cap_ = fl_bgzf_bound(in_cap_);
+    if (bam) {
+        // a child's record is smaller than its parent's plus 300 bytes (a longer name, MN:I), so one fits any batch
+        bam_ = true;
+        keep_mods_ = bam->keep_mods;
+        in_cap_ = std::max<uint64_t>(in_cap_, bam->max_record + 16);
+        out_limit_ = in_cap_ + (1u << 20);
+        out_cap_ = fl_bgzf_bound(out_limit_ + FL_BGZF_BLOCK);
+        if (fl_bam_writer_create(ctx_, &writer_bam_) != FL_OK) throw std::runtime_error(std::string("fl_bam_writer_create: ") + fl_last_error(ctx_));
+    }
     for (int i = 0; i < NIN; ++i) {
         void *p = nullptr;
         if (fl_host_alloc(in_cap_, &p) != FL_OK) { stop(); throw std::runtime_error("--bgzip: cannot allocate pinned host memory"); }
@@ -56,6 +67,16 @@ void BgzfOut::fail(const std::string &why) {
 
 void BgzfOut::put(const void *p, size_t n) {
     const char *s = (const char *)p;
+    while (bam_ && n) {                                    // raw items, at most 1 GiB each
+        uint64_t k = std::min<uint64_t>({n, in_cap_ - in_len_[fill_], out_limit_ - out_bound_, 1ull << 30});
+        if (k == 0) { submit(); continue; }
+        items_[fill_].push_back(fl_bam_item{in_len_[fill_], -1, (int32_t)k});
+        memcpy(in_[fill_] + in_len_[fill_], s, (size_t)k);
+        in_len_[fill_] += k;
+        out_bound_ += k;
+        s += k;
+        n -= (size_t)k;
+    }
     while (n) {
         const uint64_t k = std::min<uint64_t>(n, in_cap_ - in_len_[fill_]);
         memcpy(in_[fill_] + in_len_[fill_], s, (size_t)k);
@@ -64,6 +85,22 @@ void BgzfOut::put(const void *p, size_t n) {
         n -= (size_t)k;
         if (in_len_[fill_] == in_cap_) submit();
     }
+}
+
+void BgzfOut::put_child(const char *rec, int s, int e) {
+    if (!bam_) throw std::logic_error("BgzfOut::put_child on an output that is not BAM");
+    const uint64_t rb = bam_record_bytes(rec), n = (uint64_t)(e - s);
+    const uint64_t bound = rb - (uint64_t)bam_l_seq(rec) * 3 / 2 + n + n / 2 + 300;
+    if (out_bound_ + bound > out_limit_) submit();
+    if (rec != parent_) {
+        if (in_len_[fill_] + rb > in_cap_) submit();
+        parent_at_ = in_len_[fill_];
+        memcpy(in_[fill_] + parent_at_, rec, (size_t)rb);
+        in_len_[fill_] += rb;
+        parent_ = rec;
+    }
+    items_[fill_].push_back(fl_bam_item{parent_at_, s, e});
+    out_bound_ += bound;
 }
 
 // hands the batch being filled to the compressor and waits for a free one
@@ -76,6 +113,10 @@ void BgzfOut::submit() {
     fill_ = next;
     in_busy_[fill_] = true;
     in_len_[fill_] = 0;
+    items_[fill_].clear();
+    last_[fill_] = false;
+    out_bound_ = 0;
+    parent_ = nullptr;
 }
 
 void BgzfOut::compress_loop() {
@@ -100,8 +141,11 @@ void BgzfOut::compress_loop() {
         }
         if (ok) {
             std::unique_lock<std::mutex> gl(g_compress);
-            if (fl_bgzf_compress(ctx_, in_[i], in_len_[i], out_[o], out_cap_, 0, &n) != FL_OK) {
-                const std::string why = std::string("fl_bgzf_compress: ") + fl_last_error(ctx_);
+            const int rc = bam_ ? fl_bam_writer_push(writer_bam_, in_[i], in_len_[i], items_[i].data(), items_[i].size(), keep_mods_, last_[i],
+                                                     out_[o], out_cap_, &n, counts_)
+                                : fl_bgzf_compress(ctx_, in_[i], in_len_[i], out_[o], out_cap_, 0, &n);
+            if (rc != FL_OK) {
+                const std::string why = bam_ ? std::string(fl_last_error(ctx_)) : std::string("fl_bgzf_compress: ") + fl_last_error(ctx_);
                 gl.unlock();
                 std::lock_guard<std::mutex> lk(m_);
                 fail(why);
@@ -151,13 +195,15 @@ void BgzfOut::stop() {
     if (writer_.joinable()) writer_.join();
     for (int i = 0; i < NIN; ++i) if (in_[i]) { fl_host_free(in_[i]); in_[i] = nullptr; }
     for (int i = 0; i < NOUT; ++i) if (out_[i]) { fl_host_free(out_[i]); out_[i] = nullptr; }
+    if (writer_bam_) { fl_bam_writer_destroy(writer_bam_); writer_bam_ = nullptr; }
 }
 
 bool BgzfOut::finish() {
     if (finished_) return !failed_;
     finished_ = true;
-    if (in_len_[fill_]) {
+    if (in_len_[fill_] || bam_) {                          // BAM: the last batch also compresses the bytes held back
         std::lock_guard<std::mutex> lk(m_);
+        last_[fill_] = true;
         to_compress_.push_back(fill_);
         cv_.notify_all();
     }

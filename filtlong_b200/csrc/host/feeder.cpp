@@ -410,6 +410,7 @@ struct Cuts {
     uint64_t target = chunk_target(128ull << 20);
     uint64_t max_chunk = target;            // no chunk is longer (plan_chunks never cuts later than `target` bytes on)
     uint64_t bam_header = 0;                // BAM: bytes [0, bam_header) of the input are its header
+    uint64_t bam_max_record = 0;            // BAM: its largest record
 };
 
 // A stream's plain text goes to the device while it arrives; any other stream is read to its end first, then goes as a
@@ -459,7 +460,7 @@ bool plan_input(const Source &src, Plan &plan, Cuts &cuts, const Mark &mark) {
     std::string why;
     if (src.format == FL_FORMAT_BAM) {
         if (!bam_header(f.base, f.size, &cuts.bam_header, &why) ||
-            !bam_plan_chunks(f.base, f.size, cuts.bam_header, cuts.target, plan.chunks, &cuts.max_chunk, &why))
+            !bam_plan_chunks(f.base, f.size, cuts.bam_header, cuts.target, plan.chunks, &cuts.max_chunk, &why, &cuts.bam_max_record))
             throw std::runtime_error(why);
         mark("BAM block_size chain");
     } else if (!plan_chunks(f.base, f.size, src.format, cuts.target, cuts.max_chunk, plan.chunks) || plan.chunks.empty()) {
@@ -560,6 +561,7 @@ FeederOutcome run_device_feeder(Arguments &args, Kmers &kmers, StreamInput *stre
     FeederOutcome res;
     MappedFile own;
     const Source src = choose_source(args, kmers, stream, own, mark);
+    if (args.keep_mods && src.format != FL_FORMAT_BAM) throw std::runtime_error("--keep_mods needs BAM input");
     if (!src.file) return res;
     const MappedFile &f = *src.file;
     const bool bam = src.format == FL_FORMAT_BAM;
@@ -600,7 +602,7 @@ FeederOutcome run_device_feeder(Arguments &args, Kmers &kmers, StreamInput *stre
     std::cerr << "Outputting passed long reads\n";
     std::vector<Part> parts;
     for (auto &s : shards.v) parts.push_back(Part{&s.rec, Results::of(s)});
-    const Format fmt{src.format == FL_TEXT_FASTA ? '>' : '@', src.format == FL_TEXT_FASTQ, bam, cuts.bam_header};
+    const Format fmt{src.format == FL_TEXT_FASTA ? '>' : '@', src.format == FL_TEXT_FASTQ, bam, cuts.bam_header, cuts.bam_max_record, args.keep_mods};
     fl_ctx *bgzf = args.bgzip || bam ? shards.v[0].ctx : nullptr;      // BAM in, BAM out: always BGZF (--bgzip changes nothing)
     res.exit_code = write_outputs(args, g_out_fd, f.base, parts, fmt, bgzf) ? 0 : 1;
     mark("pass 2 (slices of the mapped input)");

@@ -72,9 +72,7 @@ void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Re
         for (size_t row = rs; row < rs + (size_t)res.n_child[i]; ++row) {
             const int start = res.row_s[row], end = res.row_e[row];
             if (!pass(row) || end - start <= 0 || (size_t)end > r.len) continue;
-            std::string child;
-            bam_child_record(rec, start, end, child);
-            sink.put_owned(std::move(child));
+            sink.put_child(rec, start, end);
         }
         return;
     }
@@ -110,8 +108,20 @@ void emit_range(Sink &sink, const char *base, const Part &p, size_t lo, size_t h
     for (size_t i = lo; i < hi; ++i) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i, want);
 }
 
+// the host sinks build a child's BAM record with bam_child_record
+struct HostChildren {
+    bool keep_mods = false;
+    uint64_t counts[2] = {0, 0};
+    std::string child(const char *rec, int s, int e) {
+        std::string c;
+        const int st = bam_child_record(rec, s, e, c, keep_mods);
+        if (st) ++counts[st == FL_BAM_MODS_KEPT ? 0 : 1];
+        return c;
+    }
+};
+
 // iovecs into the mapping, written with writev()
-struct Writer {
+struct Writer : HostChildren {
     static constexpr int MAXV = 1000;
     int fd;
     struct iovec v[MAXV];
@@ -142,16 +152,18 @@ struct Writer {
         small.push_back(std::move(s));
         put(small.back().data(), small.back().size());
     }
+    void put_child(const char *rec, int s, int e) { put_owned(child(rec, s, e)); }
 };
 
-struct Sizer {
+struct Sizer : HostChildren {
     uint64_t n = 0;
     void put(const void *, size_t k) { n += k; }
     void put_owned(std::string s) { n += s.size(); }
+    void put_child(const char *rec, int s, int e) { n += child(rec, s, e).size(); }
 };
 
 // copies into a buffer of about 8 MiB; flush() writes it with pwrite() at `pos`, or with write() when pos < 0
-struct Copier {
+struct Copier : HostChildren {
     int fd;
     int64_t pos;
     std::string buf;
@@ -170,6 +182,7 @@ struct Copier {
     }
     void put(const void *p, size_t k) { buf.append((const char *)p, k); if (buf.size() >= (8u << 20)) flush(); }
     void put_owned(std::string s) { put(s.data(), s.size()); }
+    void put_child(const char *rec, int s, int e) { put_owned(child(rec, s, e)); }
 };
 
 bool finish(BgzfOut &z) {
@@ -228,20 +241,26 @@ bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &p
     return lseek(fd, base_pos + (off_t)total_out, SEEK_SET) >= 0;
 }
 
-bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want) {
+bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want,
+                     uint64_t *mods_counts) {
     fflush(stdout);
     if (bgzf) {
         // compressed offsets are not known in advance: pipe or file, the members are written in order
-        BgzfOut z(bgzf, fd);
+        const BamOut bam{fmt.bam_max_record, fmt.keep_mods};
+        BgzfOut z(bgzf, fd, fmt.bam ? &bam : nullptr);
         if (fmt.bam) z.put(base, (size_t)fmt.bam_header);
         for (const Part &p : parts) emit_range(z, base, p, 0, p.rec->n, fmt, want);
-        return finish(z);
+        const bool ok = finish(z);
+        if (mods_counts) { mods_counts[0] = z.mods_counts()[0]; mods_counts[1] = z.mods_counts()[1]; }
+        return ok;
     }
     if (fmt.bam) {
         Copier c(fd, -1);
+        c.keep_mods = fmt.keep_mods;
         c.put(base, (size_t)fmt.bam_header);
         for (const Part &p : parts) emit_range(c, base, p, 0, p.rec->n, fmt, want);
         c.flush();
+        if (mods_counts) { mods_counts[0] = c.counts[0]; mods_counts[1] = c.counts[1]; }
         return !c.failed;
     }
     struct stat st;
@@ -252,8 +271,12 @@ bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, c
 }
 
 bool write_outputs(const Arguments &args, int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf) {
-    bool ok = write_survivors(fd, base, parts, fmt, bgzf);
+    uint64_t mods[2] = {0, 0};
+    bool ok = write_survivors(fd, base, parts, fmt, bgzf, true, mods);
     if (args.failed_fd >= 0 && !report_failed_write(args, write_survivors(args.failed_fd, base, parts, fmt, bgzf, false))) ok = false;
+    if (fmt.keep_mods)
+        std::cerr << "  modification tags: re-based on " << int_to_string((long long)mods[0]) << " child reads, dropped from "
+                  << int_to_string((long long)mods[1]) << " whose parent's MM/ML/MN tags are invalid\n";
     return ok;
 }
 

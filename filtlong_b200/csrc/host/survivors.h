@@ -57,6 +57,8 @@ struct Format {
     bool quality;                 // print "+" and the quality
     bool bam = false;             // BAM records (bam.h) instead of text; then lead and quality are not used
     uint64_t bam_header = 0;      // BAM: bytes [0, bam_header) of the input are the header, written first
+    uint64_t bam_max_record = 0;  // BAM: the largest record of the input
+    bool keep_mods = false;       // BAM, --keep_mods: children keep their parent's modification tags, re-based
 };
 
 struct Part {                     // one part of the table, with its results
@@ -77,11 +79,15 @@ inline void append_child_name(std::string &out, const char *name, size_t name_le
 // when it is given. The last two are the choices write_survivors makes, callable directly. BAM (fmt.bam): the header,
 // then each kept read's record as it is and a new record for each kept child; the CLI always passes a context, without
 // one the uncompressed BAM stream is written. A second output is a second call, on its descriptor with want = false.
-bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want = true);
+// With the context the children are built on its device (bgzf_out.h). mods_counts, when given, gets the children that
+// kept modification tags and those whose parent's tags are invalid (fmt.keep_mods).
+bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf, bool want = true,
+                     uint64_t *mods_counts = nullptr);
 bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want = true);
 bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want = true);
 // Both outputs of a random-access source: the survivors to fd, then, with --failed, the other rows to args.failed_fd (a
-// failure there reported by report_failed_write). True when both were written.
+// failure there reported by report_failed_write). With fmt.keep_mods, then one stderr line with stdout's mods_counts.
+// True when both were written.
 bool write_outputs(const Arguments &args, int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, fl_ctx *bgzf);
 // Sequential: the survivors among the first n_reads records of `input` (a path, or bytes in memory), parsed again. With
 // failed_fd >= 0 the same parse also writes the other rows to failed_fd (compressed too when bgzf is given), and

@@ -118,7 +118,9 @@ enum { FL_KERNEL_SCORE_PHRED = 0, FL_KERNEL_PROBE_PAINT = 1, FL_KERNEL_KMER_STAT
        FL_KERNEL_QUAL_MASK = 4, FL_KERNEL_ROW_SCAN = 5, FL_KERNEL_QUAL_GATHER = 6, FL_KERNEL_QUAL_CHILDREN = 7,
        /* --contam: the probe of the contaminant set, the per-read count and the per-row exclusion */
        FL_KERNEL_CONTAM = 8,
-       FL_KERNEL_COUNT = 9 };
+       /* BAM output: the two passes of the child-record builder (fl_bam_build), and the BGZF compressor's kernels */
+       FL_KERNEL_BAM_BUILD = 9, FL_KERNEL_BGZF = 10,
+       FL_KERNEL_COUNT = 11 };
 int fl_ctx_enable_timing(fl_ctx *ctx, int on);
 int fl_ctx_reset_timing(fl_ctx *ctx);
 int fl_ctx_kernel_time(fl_ctx *ctx, int which, double *total_ms, uint64_t *launches);
@@ -260,6 +262,41 @@ int fl_reads_push_text(fl_ctx *ctx, const char *host_text, uint64_t n_bytes, int
  * not lie inside the chunk. */
 int fl_reads_push_bam(fl_ctx *ctx, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
                       const uint32_t *qual_off, const int32_t *len);
+/* BAM output built on the device. A batch holds BAM bytes: whole records and pieces of raw stream. Each item is one
+ * piece of the output, in order: s < 0 copies bytes [off, off + e) of the batch; s >= 0 builds the child [s, e) (0 <= s
+ * < e <= l_seq) of the record that starts at byte `off` of the batch, as bam_child_record (host/bam.h) builds it --
+ * the parent's fixed fields, read_name name_<s+1>-<e>, the slice of SEQ and QUAL, the parent's RG fields and, with
+ * keep_mods and valid modification tags, the re-based MM / ML and MN:I (fl_bam_mods.h). A record's children are
+ * consecutive items that name the same record; they are cheapest in the order of their starts. The uncompressed
+ * records are written to out[0, *n_out). counts[0]: children that kept modification tags, counts[1]: children whose
+ * parent has an MM tag and invalid tags (keep_mods only; both added to, not set). FL_ERANGE: cap is too small, *n_out
+ * holds the size needed; FL_EINVAL: an item outside the batch, a child's record whose fixed fields, read_name, CIGAR,
+ * SEQ and QUAL do not fit its block_size (or l_read_name 0), a child outside [0, l_seq), or a child name longer than a
+ * BAM record allows. Aux fields are read up to the first that does not parse. */
+typedef struct fl_bam_item {
+    uint64_t off;
+    int32_t s, e;
+} fl_bam_item;
+#define FL_BAM_MODS_KEPT 1
+#define FL_BAM_MODS_INVALID 2
+/* Host buffers. */
+int fl_bam_build(fl_ctx *ctx, const void *host_batch, uint64_t n_bytes, const fl_bam_item *items, uint64_t n_items, int keep_mods,
+                 void *host_out, uint64_t cap, uint64_t *n_out, uint64_t counts[2]);
+/* Device buffers on the context's device (the batch readable 16 bytes past n_bytes). */
+int fl_bam_build_device(fl_ctx *ctx, const void *dev_batch, uint64_t n_bytes, const fl_bam_item *dev_items, uint64_t n_items,
+                        int keep_mods, void *dev_out, uint64_t cap, uint64_t *n_out, uint64_t counts[2]);
+/* One BGZF-compressed BAM output stream built batch by batch: each push builds the batch's records on the device
+ * (fl_bam_build_device), appends them to what the stream holds back, compresses the whole FL_BGZF_BLOCK-byte blocks
+ * (fl_bgzf_compress_device) into host_out[0, *n_out) and holds back the rest on the device, so that the members are cut
+ * every FL_BGZF_BLOCK bytes of the stream whatever the batches are. The push with last != 0 compresses everything
+ * left (no EOF member). A writer uses its context on the calling thread and keeps its own device buffers; several
+ * writers may share a context, one call at a time. cap >= fl_bgzf_bound(FL_BGZF_BLOCK + the batch's built bytes); a push
+ * that returns FL_ERANGE (with the size needed in *n_out) leaves the stream as it was, and may be made again. */
+typedef struct fl_bam_writer fl_bam_writer;
+int fl_bam_writer_create(fl_ctx *ctx, fl_bam_writer **out);
+int fl_bam_writer_push(fl_bam_writer *w, const void *host_batch, uint64_t n_bytes, const fl_bam_item *items, uint64_t n_items,
+                       int keep_mods, int last, void *host_out, uint64_t cap, uint64_t *n_out, uint64_t counts[2]);
+void fl_bam_writer_destroy(fl_bam_writer *w);
 /* The reference set from a chunk of the reference FILE (replaces the kseq_read loop of Kmers::add_reference,
  * kmers.cpp:75-134, for the common layouts): same contract as fl_reads_push_text -- the chunk starts at a record boundary,
  * LF line ends, FL_TEXT_FALLBACK and nothing added otherwise -- but the records' sequences go to the 16-mer set like
