@@ -175,6 +175,7 @@ struct fl_ctx {
     unsigned long long *d_bittime = nullptr;   // first time each Bloom bit was set
     uint64_t add_counter = 0;                  // global add-stream index (kmers.cpp:109-120 order)
     bool multi_pending = false;
+    bool multi_released = false;               // the state above was freed after adds: later multiple-copy adds are refused
 
     // ---- Phred LUTs ----
     double *d_lut = nullptr;   // [0..256) q, [256..512) a = q / window_size
@@ -318,6 +319,8 @@ int fl_pack_ascii_device(fl_ctx *ctx, const uint8_t *ascii, uint64_t padded_base
 int fl_kmers_ensure_bitmap(fl_ctx *ctx, KmerSet &s);
 // multi (the reference's short-read rule) is only for ctx->ref
 int fl_kmers_add_view(fl_ctx *ctx, KmerSet &s, const BatchView &b, int multi);
+// FL_EINVAL (with a message) for a multiple-copy add after fl_kmers_release_build_state freed the counts of earlier adds
+int fl_kmers_check_multi(fl_ctx *ctx, const char *entry);
 int fl_kmers_recount(fl_ctx *ctx, KmerSet &s);
 // both sets finalised (counts and probe tables current): every push calls it before it looks at ctx->ref.n
 int fl_sets_ready(fl_ctx *ctx);

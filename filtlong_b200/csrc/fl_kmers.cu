@@ -284,7 +284,16 @@ static int ensure_multi_state(fl_ctx *ctx) {
     return FL_OK;
 }
 
+// The sightings, first-seen times and Bloom times of the adds so far are gone after fl_kmers_release_build_state: a
+// multiple-copy add would start counting from zero and miss 16-mers the reference keeps (two sightings before, two after).
+int fl_kmers_check_multi(fl_ctx *ctx, const char *entry) {
+    if (!ctx->multi_released) return FL_OK;
+    ctx->set_error(std::string(entry) + ": multiple-copy adds are not possible after fl_kmers_release_build_state");
+    return FL_EINVAL;
+}
+
 int fl_kmers_add_view(fl_ctx *ctx, KmerSet &s, const BatchView &b, int multi) {
+    if (multi) FL_TRY(fl_kmers_check_multi(ctx, "fl_kmers_add_batch(_device)"));
     if (b.n == 0) return FL_OK;
     s.added = true;
     if (s.k > 16) return fl_ck_add_view(ctx, s, b);
@@ -478,6 +487,7 @@ extern "C" int fl_kmers_release_build_state(fl_ctx *ctx) {
     if (ctx->multi_pending) FL_TRY(fl_kmers_recount(ctx, ctx->ref));
     FL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     free_multi_state(ctx);
+    if (ctx->add_counter) ctx->multi_released = true;   // nothing is lost when no multiple-copy 16-mer was added yet
     return FL_OK;
 }
 

@@ -651,6 +651,7 @@ static int add_text(fl_ctx *c, KmerSet &set, const char *entry, const char *host
     *n_bases = 0;
     *bytes_consumed = 0;
     *status = FL_TEXT_OK;
+    if (require_multiple_copies) FL_TRY(fl_kmers_check_multi(c, entry));
     if (n_bytes == 0) return FL_OK;
     TextIndex ix;
     if (format == FL_TEXT_FASTA && !c->fasta_two_line_only) FL_TRY(fasta_index(c, host_text, n_bytes, is_last_chunk, status, ix));

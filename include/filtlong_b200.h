@@ -168,7 +168,10 @@ int fl_kmers_export(fl_ctx *ctx, uint32_t *out, uint64_t cap, uint64_t *n_out);
 int fl_kmers_bitmap_dev(fl_ctx *ctx, void **dev_ptr, uint64_t *n_bytes);
 /* Must be called after the bitmap was modified externally (recounts the set). */
 int fl_kmers_bitmap_changed(fl_ctx *ctx);
-/* Releases the transient multiple-copy build state (counters, first-seen times, Bloom times). */
+/* Releases the transient multiple-copy build state (counters, first-seen times, Bloom times), after resolving it into the
+ * set. Once multiple-copy 16-mers were added, the counts of those adds are gone with it: a later add with
+ * require_multiple_copies != 0 (fl_kmers_add_batch, fl_kmers_add_batch_device, fl_kmers_add_text) returns FL_EINVAL.
+ * Assembly adds (require_multiple_copies == 0) stay allowed. */
 int fl_kmers_release_build_state(fl_ctx *ctx);
 /* How the finalised set is laid out for the probe kernel (diagnostics / measurement): info[0] = a pre-filter is in use,
  * info[1] = its flavour (bit 2: one word per table group of four 16-mers, bit 3: one word per pair, bit 4: four bits per
