@@ -277,15 +277,23 @@ class Context:
         out.update(status="fallback" if st.value else "ok", n=n.value, consumed=used.value)
         return out
 
-    def push_bam(self, chunk: bytes, seq_off, qual_off, length):
+    def push_bam(self, chunk: bytes, seq_off, qual_off, length, reverse=None):
         """fl_reads_push_bam on a chunk of inflated BAM records: per record the chunk-relative offsets of SEQ and QUAL
-        and l_seq."""
+        and l_seq. reverse (optional): per record, true when it stores its read reverse-complemented
+        (fl_reads_push_bam_strand)."""
         so = np.ascontiguousarray(seq_off, dtype=np.uint32)
         qo = np.ascontiguousarray(qual_off, dtype=np.uint32)
         ln = np.ascontiguousarray(length, dtype=np.int32)
         buf = np.frombuffer(chunk, dtype=np.uint8)
-        self._ck(self.L.fl_reads_push_bam(self.h, capi.ptr(buf), buf.size, ln.size, capi.ptr(so), capi.ptr(qo), capi.ptr(ln)),
-                 "fl_reads_push_bam")
+        if reverse is None:
+            self._ck(self.L.fl_reads_push_bam(self.h, capi.ptr(buf), buf.size, ln.size, capi.ptr(so), capi.ptr(qo), capi.ptr(ln)),
+                     "fl_reads_push_bam")
+            return
+        rv = np.ascontiguousarray(reverse, dtype=np.uint8)
+        if rv.size != ln.size:
+            raise ValueError("push_bam: one reverse flag per record")
+        self._ck(self.L.fl_reads_push_bam_strand(self.h, capi.ptr(buf), buf.size, ln.size, capi.ptr(so), capi.ptr(qo), capi.ptr(ln),
+                                                 capi.ptr(rv)), "fl_reads_push_bam_strand")
 
     def kmers_add_text(self, data: bytes, fastq=True, is_last=True, multiple_copies=False):
         """fl_kmers_add_text on one chunk of a reference file (FASTQ / FASTA text)."""

@@ -167,6 +167,7 @@ SYMBOLS = [
     ("fl_reads_push_text", C.c_int, [_P, _P, C.c_uint64, C.c_int, C.c_int, C.POINTER(TextRecords), C.POINTER(C.c_uint64),
                                      C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
     ("fl_reads_push_bam", C.c_int, [_P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    ("fl_reads_push_bam_strand", C.c_int, [_P, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _P]),
     ("fl_kmers_add_text", C.c_int,[_P, _P, C.c_uint64, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                     C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
     ("fl_host_alloc", C.c_int, [C.c_uint64, C.POINTER(_P)]),

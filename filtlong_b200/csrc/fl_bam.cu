@@ -16,16 +16,17 @@
 
 namespace {
 
-// W little-endian words of the chunk starting at byte offset o (any alignment); no word past last_word is read
+// W little-endian words of the chunk starting at byte offset o (any alignment, negative allowed); no word before word 0
+// or past last_word is read
 template <int W>
-__device__ __forceinline__ void bam_load(const uint32_t *__restrict__ t32, unsigned long long o, unsigned long long last_word, uint32_t (&out)[W]) {
-    const unsigned long long w0 = o >> 2;
+__device__ __forceinline__ void bam_load(const uint32_t *__restrict__ t32, long long o, long long last_word, uint32_t (&out)[W]) {
+    const long long w0 = o >> 2;                                          // floor, also for o < 0
     const unsigned sh = ((unsigned)o & 3u) * 8u;
-    uint32_t prev = __ldg(t32 + (w0 <= last_word ? w0 : last_word));
+    uint32_t prev = __ldg(t32 + min(max(w0, 0ll), last_word));
 #pragma unroll
     for (int i = 0; i < W; ++i) {
-        const unsigned long long wi = w0 + 1 + i;
-        const uint32_t nxt = __ldg(t32 + (wi <= last_word ? wi : last_word));
+        const long long wi = w0 + 1 + i;
+        const uint32_t nxt = __ldg(t32 + min(max(wi, 0ll), last_word));
         out[i] = __funnelshift_r(prev, nxt, sh);
         prev = nxt;
     }
@@ -33,28 +34,47 @@ __device__ __forceinline__ void bam_load(const uint32_t *__restrict__ t32, unsig
 
 // 2-bit arena code of a 4-bit SEQ code, two bits per code: C (2) -> 1, G (4) -> 2, T (8) -> 3, everything else -> 0
 #define BAM_NIBBLE_CODES 0x30210u
+// the same for the complement: A (1) -> 3, C (2) -> 2, G (4) -> 1, T (8) -> 0, everything else -> 0
+#define BAM_NIBBLE_RC_CODES 0x0012Cu
 
 // One warp per record, 32 bases per lane and step (like k_text_gather). Bases at or beyond the record's length are
 // written as 0 in both arenas, as the host packer leaves them.
+//
+// reverse (may be NULL: all forward): the record stores its read reverse-complemented (BAM flag 0x10), and the arena gets
+// the read in its original orientation. Arena bases [b, b + 32) then come from the stored bases [L - b - 32, L - b),
+// last first: in Phred mode the QUAL bytes in reverse order, in k-mer mode the SEQ codes in reverse order, complemented.
+// The first stored base can be odd (the codes start half a byte into the first loaded byte) and, near the read's end,
+// negative (before the record, for the first record of a chunk before the chunk: the loads clamp at word 0); every
+// arena base it would feed lies at or past L and is masked to 0.
 template <bool PHRED>
 __global__ void __launch_bounds__(256) k_bam_gather(const uint8_t *__restrict__ chunk, unsigned long long n_bytes, uint32_t n_rec,
                                                     const uint32_t *__restrict__ seq_off, const uint32_t *__restrict__ qual_off,
-                                                    const int32_t *__restrict__ len, const unsigned long long *__restrict__ off,
-                                                    uint32_t *__restrict__ seq2b, uint8_t *__restrict__ qual) {
+                                                    const int32_t *__restrict__ len, const uint8_t *__restrict__ reverse,
+                                                    const unsigned long long *__restrict__ off, uint32_t *__restrict__ seq2b,
+                                                    uint8_t *__restrict__ qual) {
     const unsigned lane = threadIdx.x & 31;
     const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
     const uint32_t *t32 = reinterpret_cast<const uint32_t *>(chunk);
-    const unsigned long long last_word = n_bytes ? (n_bytes - 1) >> 2 : 0;
+    const long long last_word = n_bytes ? (long long)((n_bytes - 1) >> 2) : 0;
     for (size_t r = warp; r < n_rec; r += n_warps) {
         const int L = len[r];
+        const bool rev = reverse && reverse[r];                          // one warp per record: uniform
         const unsigned long long dof = off[r];
         const int padded = (int)(((unsigned)L + 63u) & ~63u);
-        const unsigned long long src = PHRED ? qual_off[r] : seq_off[r];
+        const long long src = PHRED ? qual_off[r] : seq_off[r];
         for (int b = 32 * (int)lane; b < padded; b += 1024) {
             const int nv = L - b;                                         // valid bases of these 32
             if (PHRED) {
                 uint32_t c[8];
-                bam_load<8>(t32, src + (unsigned long long)b, last_word, c);
+                bam_load<8>(t32, src + (rev ? nv - 32 : b), last_word, c);
+                if (rev) {
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const uint32_t t = c[i];
+                        c[i] = __byte_perm(c[7 - i], 0, 0x0123);
+                        c[7 - i] = __byte_perm(t, 0, 0x0123);
+                    }
+                }
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
                     const int keep = nv - 4 * i;
@@ -66,16 +86,41 @@ __global__ void __launch_bounds__(256) k_bam_gather(const uint8_t *__restrict__ 
                 dst[1] = make_uint4(c[4], c[5], c[6], c[7]);
             } else {
                 uint32_t c[4];                                            // 16 bytes = 32 codes, base 2j in the high nibble of byte j
-                bam_load<4>(t32, src + (unsigned long long)(b >> 1), last_word, c);
                 uint32_t w[2] = {0u, 0u};
+                if (!rev) {
+                    bam_load<4>(t32, src + (b >> 1), last_word, c);
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
+                    for (int i = 0; i < 4; ++i) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint32_t byte = (c[i] >> (8 * k)) & 0xFFu;
-                        const int q = 8 * i + 2 * k;                      // base of the high nibble, 0..30
-                        const uint32_t hi = (BAM_NIBBLE_CODES >> (2 * (byte >> 4))) & 3u, lo = (BAM_NIBBLE_CODES >> (2 * (byte & 15u))) & 3u;
-                        w[q >> 4] |= ((hi << 2) | lo) << (28 - 2 * (q & 15));
+                        for (int k = 0; k < 4; ++k) {
+                            const uint32_t byte = (c[i] >> (8 * k)) & 0xFFu;
+                            const int q = 8 * i + 2 * k;                  // base of the high nibble, 0..30
+                            const uint32_t hi = (BAM_NIBBLE_CODES >> (2 * (byte >> 4))) & 3u, lo = (BAM_NIBBLE_CODES >> (2 * (byte & 15u))) & 3u;
+                            w[q >> 4] |= ((hi << 2) | lo) << (28 - 2 * (q & 15));
+                        }
+                    }
+                } else {
+                    // stored codes from n0 = 2 * src + nv - 32 on (a code index); the 16 bytes from code n0 & ~1 give arena
+                    // bases 31 - q for their codes q; an odd n0 moves them one base on, and base 0 is then the high code of
+                    // the 17th byte
+                    const long long n0 = 2 * src + nv - 32;
+                    bam_load<4>(t32, n0 >> 1, last_word, c);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            const uint32_t byte = (c[i] >> (8 * k)) & 0xFFu;
+                            const int q = 31 - (8 * i + 2 * k);           // arena base of the high nibble, 31..1
+                            const uint32_t hi = (BAM_NIBBLE_RC_CODES >> (2 * (byte >> 4))) & 3u, lo = (BAM_NIBBLE_RC_CODES >> (2 * (byte & 15u))) & 3u;
+                            w[q >> 4] |= hi << (30 - 2 * (q & 15));
+                            w[(q - 1) >> 4] |= lo << (30 - 2 * ((q - 1) & 15));
+                        }
+                    }
+                    if (n0 & 1) {
+                        const long long wb = (n0 >> 1) + 16;                     // the 17th byte
+                        const uint32_t byte = (__ldg(t32 + min(max(wb >> 2, 0ll), last_word)) >> (8 * (unsigned)(wb & 3))) & 0xFFu;
+                        w[1] = __funnelshift_r(w[1], w[0], 2);
+                        w[0] = (w[0] >> 2) | (((BAM_NIBBLE_RC_CODES >> (2 * (byte >> 4))) & 3u) << 30);
                     }
                 }
                 if (nv < 32) {
@@ -334,15 +379,18 @@ __global__ void __launch_bounds__(256) k_bam_build(const uint8_t *__restrict__ b
 
 }  // namespace
 
-extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
-                                 const uint32_t *qual_off, const int32_t *len) {
-    FL_ENTER(c);
+namespace {
+
+// fl_reads_push_bam and fl_reads_push_bam_strand; what: the entry point's name, for its messages
+int push_bam(fl_ctx *c, const char *what, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
+             const uint32_t *qual_off, const int32_t *len, const uint8_t *reverse) {
+    const std::string fn(what);
     if ((!chunk && n_bytes) || (n_rec && (!chunk || !seq_off || !qual_off || !len))) {
-        c->set_error("fl_reads_push_bam: bad arguments");
+        c->set_error(fn + ": bad arguments");
         return FL_EINVAL;
     }
-    if (n_bytes >= ((uint64_t)1 << 31)) { c->set_error("fl_reads_push_bam: a chunk must be smaller than 2 GiB"); return FL_ERANGE; }
-    if (n_rec > 0xFFFFFFF0ull) { c->set_error("fl_reads_push_bam: too many records in one chunk"); return FL_ERANGE; }
+    if (n_bytes >= ((uint64_t)1 << 31)) { c->set_error(fn + ": a chunk must be smaller than 2 GiB"); return FL_ERANGE; }
+    if (n_rec > 0xFFFFFFF0ull) { c->set_error(fn + ": too many records in one chunk"); return FL_ERANGE; }
     if (n_rec == 0) return FL_OK;
     FL_TRY(fl_sets_ready(c));
     const bool kmer_mode = c->ref.n > 0;
@@ -354,15 +402,15 @@ extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes,
     for (size_t i = 0; i < n; ++i) {
         const uint64_t L = (uint64_t)(len[i] < 0 ? 0 : len[i]);
         if (len[i] < 1 || (uint64_t)seq_off[i] + (L + 1) / 2 > n_bytes || (uint64_t)qual_off[i] + L > n_bytes) {
-            c->set_error("fl_reads_push_bam: record " + std::to_string(i) + " does not lie inside the chunk");
+            c->set_error(fn + ": record " + std::to_string(i) + " does not lie inside the chunk");
             return FL_EINVAL;
         }
         off[i] = padded_bases;
         padded_bases += (L + FL_ALIGN_BASES - 1) & ~(uint64_t)(FL_ALIGN_BASES - 1);
         bases += (int64_t)L;
     }
-    // stage: chunk + SEQ / QUAL offsets in one byte buffer, lengths and offsets in the slot's own arrays (copy stream,
-    // double buffered like fl_reads_push)
+    // stage: chunk + SEQ / QUAL offsets + reverse flags in one byte buffer, lengths and offsets in the slot's own arrays
+    // (copy stream, double buffered like fl_reads_push)
     const int slot = c->stg_next;
     c->stg_next ^= 1;
     fl_ctx::Staging &S = c->stg[slot];
@@ -371,13 +419,18 @@ extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes,
     S.in_use = false;
     cudaStream_t st = c->stream, cs = c->copy_stream;
     const size_t chunk_room = ((size_t)n_bytes + 64 + 15) & ~(size_t)15;
-    FL_CUDA(c, S.ascii.reserve(chunk_room + 8 * n, 0, cs));
+    FL_CUDA(c, S.ascii.reserve(chunk_room + 8 * n + (reverse ? n : 0), 0, cs));
     FL_CUDA(c, S.off.reserve(n + 1, 0, cs));
     FL_CUDA(c, S.len.reserve(n, 0, cs));
     uint32_t *d_seq_off = reinterpret_cast<uint32_t *>(S.ascii.p + chunk_room), *d_qual_off = d_seq_off + n;
     FL_CUDA(c, cudaMemcpyAsync(S.ascii.p, chunk, (size_t)n_bytes, cudaMemcpyHostToDevice, cs));
     FL_CUDA(c, cudaMemcpyAsync(d_seq_off, seq_off, n * sizeof(uint32_t), cudaMemcpyHostToDevice, cs));
     FL_CUDA(c, cudaMemcpyAsync(d_qual_off, qual_off, n * sizeof(uint32_t), cudaMemcpyHostToDevice, cs));
+    uint8_t *d_reverse = nullptr;
+    if (reverse) {
+        d_reverse = reinterpret_cast<uint8_t *>(d_qual_off + n);
+        FL_CUDA(c, cudaMemcpyAsync(d_reverse, reverse, n, cudaMemcpyHostToDevice, cs));
+    }
     FL_CUDA(c, cudaMemcpyAsync(S.len.p, len, n * sizeof(int32_t), cudaMemcpyHostToDevice, cs));
     FL_CUDA(c, cudaMemcpyAsync(S.off.p, off.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice, cs));
     FL_CUDA(c, cudaEventRecord(c->ev_copied, cs));
@@ -390,13 +443,13 @@ extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes,
     if (ggrid > (unsigned)c->sm_count * 16) ggrid = (unsigned)c->sm_count * 16;
     if (fl_wants_bases(c)) {                                             // k-mer mode, or a contaminant set to probe
         FL_CUDA(c, S.seq.reserve((size_t)(padded_bases >> 4) + 8, 0, st));
-        k_bam_gather<false><<<ggrid, 256, 0, st>>>(S.ascii.p, n_bytes, (uint32_t)n, d_seq_off, d_qual_off, S.len.p, d_off, S.seq.p, nullptr);
+        k_bam_gather<false><<<ggrid, 256, 0, st>>>(S.ascii.p, n_bytes, (uint32_t)n, d_seq_off, d_qual_off, S.len.p, d_reverse, d_off, S.seq.p, nullptr);
         v.seq2b = S.seq.p;
         c->launches++;
     }
     if (!kmer_mode) {
         FL_CUDA(c, S.qual.reserve((size_t)padded_bases + 64, 0, st));
-        k_bam_gather<true><<<ggrid, 256, 0, st>>>(S.ascii.p, n_bytes, (uint32_t)n, d_seq_off, d_qual_off, S.len.p, d_off, nullptr, S.qual.p);
+        k_bam_gather<true><<<ggrid, 256, 0, st>>>(S.ascii.p, n_bytes, (uint32_t)n, d_seq_off, d_qual_off, S.len.p, d_reverse, d_off, nullptr, S.qual.p);
         v.qual = S.qual.p;
         c->launches++;
     }
@@ -407,6 +460,20 @@ extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes,
     S.in_use = true;
     FL_CUDA(c, cudaStreamSynchronize(cs));                               // the caller may reuse its buffers now
     return FL_OK;
+}
+
+}  // namespace
+
+extern "C" int fl_reads_push_bam(fl_ctx *c, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
+                                 const uint32_t *qual_off, const int32_t *len) {
+    FL_ENTER(c);
+    return push_bam(c, "fl_reads_push_bam", chunk, n_bytes, n_rec, seq_off, qual_off, len, nullptr);
+}
+
+extern "C" int fl_reads_push_bam_strand(fl_ctx *c, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
+                                        const uint32_t *qual_off, const int32_t *len, const uint8_t *reverse) {
+    FL_ENTER(c);
+    return push_bam(c, "fl_reads_push_bam_strand", chunk, n_bytes, n_rec, seq_off, qual_off, len, reverse);
 }
 
 // ---- BAM output (fl_bam_build, fl_bam_writer) ----

@@ -129,6 +129,7 @@ const Opt kOpts[] = {
     {0, "gpus", true, "int", "number of GPUs to shard the read set across (default: 1; not a reference option)"},
     {0, "bgzip", false, "bgzip", "compress the output as BGZF (gzip-compatible) on the GPU (not a reference option)"},
     {0, "failed", true, "file", "write the reads that are not kept to this file (not a reference option)"},
+    {0, "aligned", false, "aligned", "BAM input may be aligned: each read is scored from its primary (or unmapped) record, and its secondary and supplementary records are kept or dropped with it (not a reference option)"},
     {0, "verbose", false, "verbose", "verbose output to stderr with info for each read"},
     {0, "version", false, "version", "display the program version and quit"},
     {'h', "help", false, "help", "display this help menu"},
@@ -146,7 +147,7 @@ void print_help(const char *prog) {
         {"score weights (control the relative contribution of each score to the final read score):", 9, 11},
         {"contaminant removal:", 12, 14},
         {"read manipulation:", 15, 18},
-        {"other:", 19, 25},
+        {"other:", 19, 26},
     };
     for (const Group &g : groups) {
         o << g.title << "\n";
@@ -197,6 +198,7 @@ Arguments::Arguments(int argc, char **argv) {
         else if (ln == "gpus") gpus = (int)read_plain_ll(nm, v);
         else if (ln == "bgzip") bgzip = true;
         else if (ln == "failed") { failed = v; failed_set = true; }
+        else if (ln == "aligned") aligned = true;
         else if (ln == "verbose") verbose = true;
         else if (ln == "version") version_flag = true;
         else if (ln == "help") throw HelpRequested();
@@ -267,6 +269,7 @@ Arguments::Arguments(int argc, char **argv) {
     if (trim_q > 0 && some_reference) FAIL("Error: --trim_q cannot be used with an assembly or read reference");
     if (trim_q > 0 && !trim && !split_set) FAIL("Error: --trim_q needs --trim or --split");
     if (keep_mods && !trim && !split_set) FAIL("Error: --keep_mods needs --trim or --split");
+    if (aligned && (trim || split_set)) FAIL("Error: --aligned cannot be used with --trim or --split");
     if (trim && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --trim");
     if (split_set && !some_reference && trim_q == 0) FAIL("Error: assembly or read reference is required to use --split");
     if (max_contam_set && !contam_set) FAIL("Error: --max_contam needs --contam");

@@ -53,6 +53,7 @@ public:
     int gpus = 1;                 // this build only: shard the read set across this many GPUs (one context + one thread each)
     bool bgzip = false;           // this build only: stdout compressed as BGZF on the GPU (bgzf_out.h)
     bool keep_mods = false;       // this build only: BAM children keep their parent's MM / ML tags, re-based (fl_bam_mods.h)
+    bool aligned = false;         // this build only: BAM input may be aligned; secondary / supplementary records follow their read
     // this build only: the rows stdout does not get go to this file, opened (O_TRUNC) while the arguments are checked
     bool failed_set = false;
     std::string failed;

@@ -90,11 +90,13 @@ bool bam_plan_chunks(const char *b, uint64_t size, uint64_t header_end, uint64_t
     return true;
 }
 
-bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix) {
+bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix, bool aligned) {
     Records &R = ix.rec;
     R.n = 0;
     ix.seq32.clear();
     ix.qual32.clear();
+    ix.reverse.clear();
+    ix.followers.clear();
     ix.error.clear();
     const char *base = b + c.begin;
     uint64_t p = 0;
@@ -122,28 +124,85 @@ bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix) {
             }
         }
         const std::string shown(name, l_name - 1);
-        if (!(flag & 0x4) || (flag & 0x910) || n_cigar != 0) {
+        const bool follower = aligned && (flag & 0x900);
+        if (!aligned && (!(flag & 0x4) || (flag & 0x910) || n_cigar != 0)) {
             ix.error = "BAM input must be unaligned: read " + shown + " has flag " + std::to_string(flag) + " and " +
                        std::to_string(n_cigar) + " CIGAR operations";
             return false;
         }
-        if (l_seq < 1) {
+        if (!follower && l_seq < 1) {
             ix.error = "BAM read " + shown + " has no sequence";
             return false;
+        }
+        if (aligned && !follower && !(flag & 0x4)) {                           // mapped: the record must hold the whole read
+            uint64_t query = 0;
+            bool hard = false;
+            for (uint64_t k = 0; k < n_cigar; ++k) {
+                const uint32_t op = u32(name + l_name + 4 * k), code = op & 15u;
+                if (code > 8) {
+                    ix.error = "BAM read " + shown + " has a CIGAR operation of code " + std::to_string(code);
+                    return false;
+                }
+                hard = hard || code == 5;
+                if (code == 0 || code == 1 || code == 4 || code == 7 || code == 8) query += op >> 4;   // M I S = X
+            }
+            if (hard) {
+                ix.error = "BAM read " + shown + ": its primary record is hard-clipped";
+                return false;
+            }
+            if (query != l_seq) {
+                ix.error = "BAM read " + shown + ": the query length of its CIGAR (" + std::to_string(query) + ") is not its l_seq (" +
+                           std::to_string(l_seq) + ")";
+                return false;
+            }
         }
         for (uint64_t i = 0; i + 1 < l_name; ++i)
             if ((unsigned char)name[i] < '!' || (unsigned char)name[i] > '~') {
                 ix.error = "BAM read name with a byte outside '!'..'~' in the " + at_byte(at);
                 return false;
             }
+        if (follower) {
+            ix.followers.push_back(Follower{p, R.n, fl_name_hash((const unsigned char *)name, l_name - 1)});
+            p += 4 + bs;
+            continue;
+        }
         const uint64_t name_off = (uint64_t)(name - base), seq_off = (uint64_t)(seq - base), qual_off = (uint64_t)(qual - base);
         R.add(name_off, (uint32_t)(l_name - 1), 0, seq_off, qual_off, (int32_t)l_seq);
         R.name_hash[R.n - 1] = fl_name_hash((const unsigned char *)name, l_name - 1);
         ix.seq32.push_back((uint32_t)seq_off);
         ix.qual32.push_back((uint32_t)qual_off);
+        if (aligned) ix.reverse.push_back((flag & 0x10) ? 1 : 0);
         p += 4 + bs;
     }
     return true;
+}
+
+void bam_append_chunk(const BamChunkIndex &ix, const Chunk &c, Records &R, std::vector<Follower> &F, std::vector<uint8_t> *rev) {
+    const Records &X = ix.rec;
+    for (Follower f : ix.followers) {
+        f.off += c.begin;
+        f.before += R.n;
+        F.push_back(f);
+    }
+    R.ensure(R.n + X.n);
+    for (size_t j = 0; j < X.n; ++j, ++R.n) {
+        R.name_off[R.n] = X.name_off[j] + c.begin; R.seq_off[R.n] = X.seq_off[j] + c.begin; R.qual_off[R.n] = X.qual_off[j] + c.begin;
+        R.name_len[R.n] = X.name_len[j]; R.comment_len[R.n] = 0; R.len[R.n] = X.len[j]; R.name_hash[R.n] = X.name_hash[j];
+    }
+    if (rev) rev->insert(rev->end(), ix.reverse.begin(), ix.reverse.end());
+}
+
+uint64_t bam_join_followers(const char *b, const NameIndex &names, std::vector<Follower> &F) {
+    uint64_t orphans = 0;
+    for (Follower &f : F) {
+        const char *rec = b + f.off;
+        f.owner_part = -1;
+        if (!names.find(f.name_hash, rec + kFixed, (uint32_t)(uint8_t)rec[kLReadName] - 1, &f.owner_part, &f.owner)) {
+            f.owner_part = -1;
+            ++orphans;
+        }
+    }
+    return orphans;
 }
 
 uint64_t bam_record_bytes(const char *rec) { return 4 + (uint64_t)u32(rec); }

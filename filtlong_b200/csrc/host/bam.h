@@ -1,5 +1,5 @@
-// filtlong_b200/csrc/host/bam.h -- unaligned BAM input: the only code that knows the BAM record layout (SAM/BAM format
-// specification, section 4.2).
+// filtlong_b200/csrc/host/bam.h -- BAM input, unaligned or (--aligned) aligned: the only code that knows the BAM record
+// layout (SAM/BAM format specification, section 4.2).
 //
 // A BAM file is BGZF; it is inflated into memory like any gzip input (textsrc.h, gzmem.h), and an inflated input that
 // starts with "BAM\1" is this format (MappedFile::format() == FL_FORMAT_BAM). The header is copied to the output as it
@@ -39,13 +39,28 @@ bool bam_plan_chunks(const char *b, uint64_t size, uint64_t header_end, uint64_t
 struct BamChunkIndex {
     Records rec;
     std::vector<uint32_t> seq32, qual32;
+    std::vector<uint8_t> reverse;         // aligned: per read record, 1 when it is reverse-complemented (flag 0x10)
+    std::vector<Follower> followers;      // aligned: the secondary and supplementary records (`before` counts rec)
     std::string error;            // why the first record that failed a check failed (then the index stops there)
 };
 
 // Checks and indexes the records of chunk c of the inflated input b: fields inside the record, aux fields that parse up
 // to its end, unaligned (flag 0x4 set, 0x10 / 0x100 / 0x800 clear, no CIGAR), l_seq >= 1, name bytes in '!'..'~'.
 // false: ix.error says why, naming the record by its byte offset in the inflated input or by its read name.
-bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix);
+//
+// aligned (--aligned): records may be aligned. A record with flag & 0x900 == 0 is a read record, indexed in ix.rec with
+// its reverse flag; it needs l_seq >= 1 and, when mapped (0x4 clear), a CIGAR without H whose query length (M I S = X)
+// is l_seq, so that the record holds the whole read. Any other record is a follower (ix.followers): it is not scored
+// and may have no SEQ. Both get the checks every record gets.
+bool bam_index_chunk(const char *b, const Chunk &c, BamChunkIndex &ix, bool aligned = false);
+
+// Appends chunk c's index to a part's tables, as file offsets: its read records to R (their reverse flags to rev when
+// given), its followers to F, counted among R's reads.
+void bam_append_chunk(const BamChunkIndex &ix, const Chunk &c, Records &R, std::vector<Follower> &F, std::vector<uint8_t> *rev = nullptr);
+
+// Finds each follower's read record by name (names: the parts' Records, in order) and sets its owner; returns the
+// number of orphans.
+uint64_t bam_join_followers(const char *b, const NameIndex &names, std::vector<Follower> &F);
 
 // the record whose read_name starts at `name`: its first byte (block_size) and its size
 inline const char *bam_record_of(const char *name) { return name - 36; }

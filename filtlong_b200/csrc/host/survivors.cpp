@@ -29,6 +29,51 @@ bool Records::within(uint64_t file_size, bool quality) const {
     return true;
 }
 
+bool NameIndex::build(const std::vector<const Records *> &tables, const char *base, std::string *dup) {
+    tables_ = tables;
+    base_ = base;
+    size_t n = 0;
+    for (const Records *t : tables) n += t->n;
+    size_t cap = 16;
+    while (cap < 2 * n + 16) cap <<= 1;
+    keys_.assign(cap, 0);
+    at_.assign(cap, 0);
+    mask_ = cap - 1;
+    for (size_t t = 0; t < tables.size(); ++t) {
+        const Records &R = *tables[t];
+        for (size_t i = 0; i < R.n; ++i) {
+            const uint64_t h = R.name_hash[i];
+            size_t slot = (size_t)(h * 0x9E3779B97F4A7C15ull) & mask_;
+            for (; at_[slot]; slot = (slot + 1) & mask_) {
+                if (keys_[slot] != h) continue;
+                const Records &O = *tables[(at_[slot] - 1) >> 56];
+                const uint64_t j = (at_[slot] - 1) & ((1ull << 56) - 1);
+                if (O.name_len[j] == R.name_len[i] && memcmp(base + O.name_off[j], base + R.name_off[i], R.name_len[i]) == 0) {
+                    dup->assign(base + R.name_off[i], R.name_len[i]);
+                    return false;
+                }
+            }
+            keys_[slot] = h;
+            at_[slot] = ((uint64_t)t << 56 | i) + 1;
+        }
+    }
+    return true;
+}
+
+bool NameIndex::find(uint64_t h, const char *name, uint32_t len, int32_t *table, uint64_t *index) const {
+    for (size_t slot = (size_t)(h * 0x9E3779B97F4A7C15ull) & mask_; at_[slot]; slot = (slot + 1) & mask_) {
+        if (keys_[slot] != h) continue;
+        const uint64_t t = (at_[slot] - 1) >> 56, i = (at_[slot] - 1) & ((1ull << 56) - 1);
+        const Records &R = *tables_[t];
+        if (R.name_len[i] == len && memcmp(base_ + R.name_off[i], name, len) == 0) {
+            *table = (int32_t)t;
+            *index = i;
+            return true;
+        }
+    }
+    return false;
+}
+
 namespace {
 
 struct RecordText {               // one input record's bytes
@@ -103,9 +148,30 @@ void emit_survivors(Sink &sink, const Format &fmt, const RecordText &r, const Re
     }
 }
 
+// Reads [lo, hi) of part pi. BAM --aligned: with each read, in file order, the followers just before it, and after the
+// part's last read those after it; a follower is written when its read's pass flag is `want`, an orphan when want is
+// false.
 template <class Sink>
-void emit_range(Sink &sink, const char *base, const Part &p, size_t lo, size_t hi, const Format &fmt, bool want) {
-    for (size_t i = lo; i < hi; ++i) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i, want);
+void emit_range(Sink &sink, const char *base, const std::vector<Part> &parts, size_t pi, size_t lo, size_t hi, const Format &fmt, bool want) {
+    const Part &p = parts[pi];
+    if (!p.followers) {
+        for (size_t i = lo; i < hi; ++i) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i, want);
+        return;
+    }
+    const std::vector<Follower> &F = *p.followers;
+    auto f = std::lower_bound(F.begin(), F.end(), lo, [](const Follower &x, size_t i) { return x.before < i; });
+    const bool last = hi == p.rec->n;                                   // the part's last range also takes those after its reads
+    for (size_t i = lo; i < hi || (last && i == hi); ++i) {
+        for (; f != F.end() && f->before == i; ++f) {
+            bool kept = false;
+            if (f->owner_part >= 0) {
+                const Results &r = parts[(size_t)f->owner_part].res;
+                kept = r.row_pfinal[r.row_start[f->owner]] != 0;
+            }
+            if (kept == want) sink.put(base + f->off, bam_record_bytes(base + f->off));
+        }
+        if (i < hi) emit_survivors(sink, fmt, text_of(*p.rec, base, i), p.res, i, want);
+    }
 }
 
 // the host sinks build a child's BAM record with bam_child_record
@@ -195,7 +261,7 @@ bool finish(BgzfOut &z) {
 
 bool write_survivors_writev(int fd, const char *base, const std::vector<Part> &parts, const Format &fmt, bool want) {
     Writer w(fd);
-    for (const Part &p : parts) emit_range(w, base, p, 0, p.rec->n, fmt, want);
+    for (size_t pi = 0; pi < parts.size(); ++pi) emit_range(w, base, parts, pi, 0, parts[pi].rec->n, fmt, want);
     w.flush();
     return !w.failed;
 }
@@ -221,11 +287,11 @@ bool write_survivors_pwrite(int fd, const char *base, const std::vector<Part> &p
                     Group &G = groups[g];
                     if (!write_pass) {
                         Sizer z;
-                        emit_range(z, base, parts[G.part], G.lo, G.hi, fmt, want);
+                        emit_range(z, base, parts, G.part, G.lo, G.hi, fmt, want);
                         G.bytes = z.n;
                     } else {
                         Copier c(fd, (int64_t)base_pos + (int64_t)G.at);
-                        emit_range(c, base, parts[G.part], G.lo, G.hi, fmt, want);
+                        emit_range(c, base, parts, G.part, G.lo, G.hi, fmt, want);
                         c.flush();
                         if (c.failed) bad.store(true);
                     }
@@ -249,7 +315,7 @@ bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, c
         const BamOut bam{fmt.bam_max_record, fmt.keep_mods};
         BgzfOut z(bgzf, fd, fmt.bam ? &bam : nullptr);
         if (fmt.bam) z.put(base, (size_t)fmt.bam_header);
-        for (const Part &p : parts) emit_range(z, base, p, 0, p.rec->n, fmt, want);
+        for (size_t pi = 0; pi < parts.size(); ++pi) emit_range(z, base, parts, pi, 0, parts[pi].rec->n, fmt, want);
         const bool ok = finish(z);
         if (mods_counts) { mods_counts[0] = z.mods_counts()[0]; mods_counts[1] = z.mods_counts()[1]; }
         return ok;
@@ -258,7 +324,7 @@ bool write_survivors(int fd, const char *base, const std::vector<Part> &parts, c
         Copier c(fd, -1);
         c.keep_mods = fmt.keep_mods;
         c.put(base, (size_t)fmt.bam_header);
-        for (const Part &p : parts) emit_range(c, base, p, 0, p.rec->n, fmt, want);
+        for (size_t pi = 0; pi < parts.size(); ++pi) emit_range(c, base, parts, pi, 0, parts[pi].rec->n, fmt, want);
         c.flush();
         if (mods_counts) { mods_counts[0] = c.counts[0]; mods_counts[1] = c.counts[1]; }
         return !c.failed;

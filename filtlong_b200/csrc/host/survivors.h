@@ -61,9 +61,36 @@ struct Format {
     bool keep_mods = false;       // BAM, --keep_mods: children keep their parent's modification tags, re-based
 };
 
+// BAM --aligned: a secondary or supplementary record. It is not scored; it is written when its read record (the one of
+// the same name) is, and an orphan (no read record has its name) only to --failed.
+struct Follower {
+    uint64_t off;                 // its first byte (block_size), a file offset
+    uint64_t before;              // the index in its part's Records of the read record after it (Records::n: none)
+    uint64_t name_hash;           // fl_name_hash of its read_name
+    int32_t owner_part = -1;      // its read record: part, and index in that part's Records; -1: an orphan
+    uint64_t owner = 0;
+};
+
 struct Part {                     // one part of the table, with its results
     const Records *rec;
     Results res;
+    const std::vector<Follower> *followers = nullptr;   // BAM --aligned: in file order
+};
+
+// The read names of one or more tables: a flat open-addressing table over the 64-bit hashes computed with the records,
+// names compared byte for byte in the input only when two hashes agree; no string is built.
+class NameIndex {
+public:
+    // tables[t] in order; false: *dup is the first name met twice (the table is then incomplete)
+    bool build(const std::vector<const Records *> &tables, const char *base, std::string *dup);
+    // the record named name[0, len) whose hash is h: true, *table and *index set
+    bool find(uint64_t h, const char *name, uint32_t len, int32_t *table, uint64_t *index) const;
+
+private:
+    std::vector<const Records *> tables_;
+    const char *base_ = nullptr;
+    std::vector<uint64_t> keys_, at_;          // at_: (table << 56 | index) + 1, 0 for a free slot
+    size_t mask_ = 0;
 };
 
 // name_<start+1>-<end>, a child read's name (reference src/read.cpp:135-136), appended to `out`

@@ -265,6 +265,12 @@ int fl_reads_push_text(fl_ctx *ctx, const char *host_text, uint64_t n_bytes, int
  * not lie inside the chunk. */
 int fl_reads_push_bam(fl_ctx *ctx, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
                       const uint32_t *qual_off, const int32_t *len);
+/* Aligned BAM input: the same, with reverse[i] != 0 for a record that stores its read reverse-complemented (flag 0x10).
+ * Such a record is scored as the read in its original orientation, as `samtools fastq` writes it: QUAL reversed, SEQ
+ * reversed and complemented (A <-> T, C <-> G, every other code counts as a base outside ACGT). reverse == NULL: every
+ * record is forward, as with fl_reads_push_bam. */
+int fl_reads_push_bam_strand(fl_ctx *ctx, const char *chunk, uint64_t n_bytes, uint64_t n_rec, const uint32_t *seq_off,
+                             const uint32_t *qual_off, const int32_t *len, const uint8_t *reverse);
 /* BAM output built on the device. A batch holds BAM bytes: whole records and pieces of raw stream. Each item is one
  * piece of the output, in order: s < 0 copies bytes [off, off + e) of the batch; s >= 0 builds the child [s, e) (0 <= s
  * < e <= l_seq) of the record that starts at byte `off` of the batch, as bam_child_record (host/bam.h) builds it --
