@@ -499,10 +499,11 @@ __global__ void k_phred_fill(const int32_t *__restrict__ len, uint32_t n, int ws
 #define PT_THREADS 256
 #define PT_SMEM (256 * 16 * 8)         // one table, 16 lane-private copies = 32 KiB
 #define PS_TILE 512
-// Blocks per SM of k_phred_sum. Three, not the four its shared memory allows: capped at 64 registers the compiler keeps
-// the prefetched uint4 on the stack, and the store that puts it there waits for the load -- every step then pays a full
-// global round trip before it computes. With 85 registers to use (80 used) the load stays in flight during the step.
-#define PS_OCC 3
+// Blocks per SM of k_phred_sum: four, at 63 registers and no spill. The crossing replay reads its table entries again
+// (volatile) instead of reusing the step's 16 gathered doubles; reusing them kept those 32 registers live into the
+// replay, and under the 64-register cap of four blocks the compiler then spilled the prefetched uint4, whose store
+// waits for the load (every step a full global round trip), or, at three blocks, took 80 registers.
+#define PS_OCC 4
 
 struct TieInfo {
     unsigned long long any;            // bit e: some table value q ties when added to a sum in [2^e, 2^(e+1))
@@ -678,7 +679,7 @@ __global__ void __launch_bounds__(PT_THREADS, PS_OCC) k_phred_sum(PhredArgs a, T
                     double v = (int)lane == lx ? t0 : C;
                     if ((int)lane >= lx) {
 #pragma unroll
-                        for (int k = 0; k < 16; ++k) v += *entry_of(tl, cw[k >> 2], k & 3);
+                        for (int k = 0; k < 16; ++k) v += *(const volatile double *)entry_of(tl, cw[k >> 2], k & 3);   // (see PS_OCC)
                     }
                     const double t = shfl_d(v, lx);
                     bool hit = false;

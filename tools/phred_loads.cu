@@ -7,6 +7,9 @@
 //   MODE 0  one step ahead in registers: a uint4 per lane (KIND 0), three clamped 32-bit words per lane (KIND 1)
 //   MODE 1  a ring of D tiles of 512 bytes per warp in shared memory, filled by lane 0 with cp.async.bulk
 //   MODE 2  the same ring, filled by every lane with 16-byte cp.async
+//   MODE 3  (KIND 0 only) what k_phred_sum does: D private 16-byte slots per lane, each lane copying its own chunk of
+//           the step D ahead with cp.async and one commit group per step, cp.async.wait_group D-1 before reading a
+//           slot; no barrier, no producer lane, a cold start per read
 // DEEP: the warp holds the next read's descriptor while it walks this one, the ring is refilled across the read
 // boundary, and short reads are claimed eight per atomicAdd. Without it a read starts cold.
 // k_chunked (below): the same walks cut into chunks, with a bulk L2 prefetch ahead, and both walks in one pass.
@@ -158,7 +161,39 @@ __global__ void __launch_bounds__(THREADS) k_probe(Args a) {
     for (int i = threadIdx.x; i < a.table_bytes / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem_raw)[i] = 0u;
     __syncthreads();
     const int skip = KIND == 0 ? H : WS;
-    if (MODE == 0) {
+    if constexpr (MODE == 3) {
+        static_assert(KIND == 0, "per-lane slots: k_phred_sum's walk only");
+        const uint32_t slot0 = (uint32_t)__cvta_generic_to_shared(smem_raw + a.table_bytes) + 16u * threadIdx.x;
+        for (;;) {
+            unsigned long long it = 0;
+            if (lane == 0) it = atomicAdd(a.work, 1ull);
+            it = __shfl_sync(FULL, it, 0);
+            if (it >= a.n) break;
+            const uint32_t r = a.order[it];
+            const int L = a.len[r];
+            if (L <= skip) continue;
+            const uint8_t *ql = a.qual + a.off[r] + 16 * lane;
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                if (TILE * d + 16 * (int)lane < L - H)
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(slot0 + d * (THREADS * 16)), "l"(ql + H + TILE * d) : "memory");
+                asm volatile("cp.async.commit_group;" ::: "memory");
+            }
+            uint32_t x = 0, slot = slot0;
+            for (int j = H; j < L; j += TILE) {
+                uint32_t c0, c1, c2, c3;
+                asm volatile("cp.async.wait_group %4;\n\tld.shared.v4.u32 {%0, %1, %2, %3}, [%5];"
+                             : "=r"(c0), "=r"(c1), "=r"(c2), "=r"(c3) : "n"(D - 1), "r"(slot) : "memory");
+                if (D * TILE + 16 * (int)lane < L - j)
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(slot), "l"(ql + j + D * TILE) : "memory");
+                asm volatile("cp.async.commit_group;" ::: "memory");
+                slot = slot == slot0 + (D - 1) * (THREADS * 16) ? slot0 : slot + THREADS * 16;
+                x ^= c0 ^ c1 ^ c2 ^ c3;          // (a lane past the read's end reads a stale slot: not compared either)
+            }
+            x = __reduce_xor_sync(FULL, x);
+            if (lane == 0) a.out[r] = x;
+        }
+    } else if (MODE == 0) {
         for (;;) {
             unsigned long long it = 0;
             if (lane == 0) it = atomicAdd(a.work, 1ull);
@@ -363,5 +398,6 @@ extern "C" int probe_launch(int kind, int mode, int depth, int deep, int occ, co
     KINDS(1, 2, false) KINDS(1, 4, false) KINDS(1, 8, false)
     KINDS(1, 2, true) KINDS(1, 4, true) KINDS(1, 8, true)
     KINDS(2, 2, true) KINDS(2, 4, true) KINDS(2, 8, true)
+    CASE(0, 3, 2, false) CASE(0, 3, 3, false) CASE(0, 3, 4, false)
     return -1;
 }

@@ -8,7 +8,8 @@ kernel waiting for its loads.
 Part 2, load-only probes (tools/phred_loads.cu, compiled here with the library's nvcc flags into a temporary directory,
 never linked into the library): the same claim loop, addresses and shared-memory footprint as each kernel, the per-base
 work replaced by an XOR. Variants: loads one step ahead in registers; a per-warp shared-memory ring of 2, 4 or 8 tiles
-filled by cp.async.bulk or by per-lane cp.async; reads taken longest first or in arena order; the next read claimed
+filled by cp.async.bulk or by per-lane cp.async; for k_phred_sum's walk alone, the per-lane slots the kernel uses (2, 3
+or 4 steps ahead, a cold start per read); reads taken longest first or in arena order; the next read claimed
 and prefetched while this one is walked, or not. Then the chunked walks, with the shared-memory footprint of a
 one-pass kernel that would hold both chains' tables (72 KiB, three blocks per SM): each read cut into chunks of 2, 4 or
 8 KiB, lane 0 asking L2 for the chunk D = 1 or 2 ahead with cp.async.bulk.prefetch.L2 (D = 0: no prefetch), the loads
@@ -117,7 +118,9 @@ VARIANTS = [("registers, one step ahead", 0, 1, 0, 1), ("registers, arena order"
             ("bulk ring 4, cold start per read", 1, 4, 0, 1),
             ("bulk ring 2", 1, 2, 1, 1), ("bulk ring 4", 1, 4, 1, 1), ("bulk ring 8", 1, 8, 1, 1),
             ("bulk ring 4, arena order", 1, 4, 1, 0),
-            ("cp.async ring 2", 2, 2, 1, 1), ("cp.async ring 4", 2, 4, 1, 1), ("cp.async ring 8", 2, 8, 1, 1)]
+            ("cp.async ring 2", 2, 2, 1, 1), ("cp.async ring 4", 2, 4, 1, 1), ("cp.async ring 8", 2, 8, 1, 1),
+            ("per-lane slots 2 (k_phred_sum's only)", 3, 2, 0, 1), ("per-lane slots 3", 3, 3, 0, 1),
+            ("per-lane slots 4", 3, 4, 0, 1)]
 
 
 def probe_part(torch, dev, stream, args):
@@ -140,6 +143,10 @@ def probe_part(torch, dev, stream, args):
                 order = longest if by_length else arena
                 cells = []
                 for kind in (0, 1):
+                    if mode == 3 and kind == 1:
+                        cells.append("-")
+                        continue
+
                     def launch():
                         rc = lib.probe_launch(kind, mode, depth, deep, 4, d_qual.data_ptr(), t_off.data_ptr(), t_len.data_ptr(),
                                               order.data_ptr(), w["n"], work.data_ptr(), out.data_ptr(), sms, stream.cuda_stream)
